@@ -23,6 +23,7 @@ namespace {
 
 thread_local std::string g_error;
 std::atomic<int64_t> g_launches{0};
+std::atomic<bool> g_chain_pdl_rejected{false};  // a PDL launch of the chain kernel failed once
 
 int fail(const std::string& msg) {
   g_error = msg;
@@ -298,12 +299,74 @@ __device__ __forceinline__ void peer_count_kernel(const PeerOut& peers) {
   }
 }
 
+// Programmatic dependent launch (PDL).  The chain kernel is one wave whose end waits for
+// its slowest warps (the few instances in Cholesky rounds); launched with the
+// programmatic-serialization attribute, the next launch on the stream starts its CTAs in
+// the slots those tail CTAs leave free.  Protocol of the PDL instantiation:
+//   - griddepcontrol.launch_dependents first: the next grid may start at once;
+//   - q and the targets row are read and solved before griddepcontrol.wait, which every
+//     valid thread executes before its first global store: no grid completes before its
+//     predecessor, so stream order holds for whatever runs after it;
+//   - the library cannot see what ran before it on the stream (our own previous call
+//     writing this call's q, or a foreign kernel that triggers early and then writes q or
+//     the targets), so after the wait the q row and the targets row are read again from L2
+//     (ld.global.cg) and compared bitwise with the values the steps used.  On a difference
+//     every step of the instance is recomputed from the re-read values.
+// The steps read the targets row from a copy in local memory, never through the read-only
+// path, so "the values the steps used" are exactly the copy, and a line the L1 cached
+// before the wait cannot leak into the recompute.
+// PK_CHAIN_PDL=0 (compile time) launches the plain instantiation only, for A/B runs.
+#ifndef PK_CHAIN_PDL
+#define PK_CHAIN_PDL 1
+#endif
+__device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
+__device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
+
+// flags bit: after the wait, recompute every instance as if its inputs had changed (tests)
+constexpr int kChainForceRecompute = 4;
+// longest targets row the PDL instantiation copies: frame targets, posture and dq_prev
 template <int NJ, int NFT>
+constexpr int kChainRowWords = 12 * NFT + 2 * NJ;
+
+template <bool CG>
+__device__ __forceinline__ float4 chain_ld4(const float* p) {
+  if constexpr (CG) return __ldcg(reinterpret_cast<const float4*>(p));
+  else return __ldg(reinterpret_cast<const float4*>(p));
+}
+// Copy the first `n` words of the targets row `src` to `dst` (local memory); returns
+// whether every word was bitwise equal to what `dst` held.  CG: read from L2.
+template <bool CG>
+__device__ __forceinline__ bool chain_copy_row(float* dst, const float* src, int n, bool v4) {
+  unsigned diff = 0u;
+  if (v4) {
+#pragma unroll 1
+    for (int k = 0; k < n; k += 4) {
+      const float4 t = chain_ld4<CG>(src + k);
+      diff |= (__float_as_uint(t.x) ^ __float_as_uint(dst[k])) | (__float_as_uint(t.y) ^ __float_as_uint(dst[k + 1])) |
+              (__float_as_uint(t.z) ^ __float_as_uint(dst[k + 2])) | (__float_as_uint(t.w) ^ __float_as_uint(dst[k + 3]));
+      dst[k] = t.x;
+      dst[k + 1] = t.y;
+      dst[k + 2] = t.z;
+      dst[k + 3] = t.w;
+    }
+  } else {
+#pragma unroll 1
+    for (int k = 0; k < n; ++k) {
+      const float t = CG ? __ldcg(src + k) : __ldg(src + k);
+      diff |= __float_as_uint(t) ^ __float_as_uint(dst[k]);
+      dst[k] = t;
+    }
+  }
+  return diff == 0u;
+}
+
+template <int NJ, int NFT, bool PDL>
 __global__ void __launch_bounds__(128, 4)
     ik_chain_kernel(const __grid_constant__ ChainParams<NJ> P, const float* __restrict__ q,
                     const float* __restrict__ targets, float* __restrict__ v, int32_t* __restrict__ status,
                     int64_t B, int flags, int n_steps, float* __restrict__ q_out,
                     const __grid_constant__ PeerOut peers) {
+  if constexpr (PDL) pdl_launch_dependents();
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   peer_gate(peers);
   if (i >= B) return;
@@ -320,21 +383,54 @@ __global__ void __launch_bounds__(128, 4)
 #pragma unroll
     for (int k = 0; k < NJ; ++k) qi[k] = __ldg(qrow + k);
   }
-  const float* trow = targets + i * (int64_t)P.target_stride;
-  int st_all = 0;
+  const float* grow = targets + i * (int64_t)P.target_stride;
+  const float* trow = grow;
+  // PDL: [targets row (target_stride <= kChainRowWords words) | q row] as the steps use them
+  __align__(16) float used[PDL ? kChainRowWords<NJ, NFT> + NJ : 1];
+  float* const used_q = used + (PDL ? kChainRowWords<NJ, NFT> : 0);
+  const bool v4 = P.target_vec4 && (reinterpret_cast<uintptr_t>(grow) & 15u) == 0u;
+  if constexpr (PDL) {
+    chain_copy_row<false>(used, grow, P.target_stride, v4);
 #pragma unroll
-  for (int k = 0; k < NJ; ++k) vi[k] = 0.f;
+    for (int k = 0; k < NJ; ++k) used_q[k] = qi[k];
+    trow = used;
+  }
+  int st_all;
 #pragma unroll 1
-  for (int step_no = 0; step_no < n_steps; ++step_no) {
-    const bool frozen =
-        (st_all & (PK_STATUS_NO_SOLUTION | PK_STATUS_NOT_POSDEF)) || ((st_all & PK_STATUS_OUT_OF_LIMITS) && P.safety_break);
-    if (frozen) break;
-    int st;
-    ik_step_chain<NJ, NFT>(P, qi, trow, vi, st, flags);
-    st_all |= st & 0xff;
-    if (n_steps > 1 || q_out) {
+  for (int pass = 0;; ++pass) {
+    st_all = 0;
 #pragma unroll
-      for (int k = 0; k < NJ; ++k) qi[k] = fmaf(vi[k], P.dt, qi[k]);  // 1-dof joints: q (+) v dt = q + v dt
+    for (int k = 0; k < NJ; ++k) vi[k] = 0.f;
+#pragma unroll 1
+    for (int step_no = 0; step_no < n_steps; ++step_no) {
+      const bool frozen =
+          (st_all & (PK_STATUS_NO_SOLUTION | PK_STATUS_NOT_POSDEF)) || ((st_all & PK_STATUS_OUT_OF_LIMITS) && P.safety_break);
+      if (frozen) break;
+      int st;
+      ik_step_chain<NJ, NFT>(P, qi, trow, vi, st, flags);
+      st_all |= st & 0xff;
+      if (n_steps > 1 || q_out) {
+#pragma unroll
+        for (int k = 0; k < NJ; ++k) qi[k] = fmaf(vi[k], P.dt, qi[k]);  // 1-dof joints: q (+) v dt = q + v dt
+      }
+    }
+    if constexpr (!PDL) {
+      break;
+    } else {
+      if (pass > 0) break;
+      pdl_wait();
+      // the inputs as the predecessors left them; one recompute at most (nothing writes
+      // them once the predecessors are complete)
+      bool same = chain_copy_row<true>(used, grow, P.target_stride, v4) && !(flags & kChainForceRecompute);
+#pragma unroll
+      for (int k = 0; k < NJ; ++k) {
+        const float t = __ldcg(qrow + k);
+        same &= __float_as_uint(t) == __float_as_uint(used_q[k]);
+        used_q[k] = t;
+      }
+      if (same) break;
+#pragma unroll
+      for (int k = 0; k < NJ; ++k) qi[k] = used_q[k];
     }
   }
   if (v) {
@@ -576,10 +672,34 @@ template <int NJ, int NFT>
 int launch_chain_nft(const pk::ChainParams<NJ>& C, const float* q, const float* targets, float* v, int32_t* status,
                      int64_t B, cudaStream_t stream, int n_steps, float* q_out, const pk::PeerOut& peers) {
   // A/B and probe switches (timing experiments; see scripts/ab.sh)
-  static const int flags = (env_int("PK_CLOSED_FORM", 1) ? 0 : 1) | (env_int("PK_PROBE_SKIP_ROUNDS", 0) ? 2 : 0);
+  static const int flags = (env_int("PK_CLOSED_FORM", 1) ? 0 : 1) | (env_int("PK_PROBE_SKIP_ROUNDS", 0) ? 2 : 0) |
+                           (env_int("PK_CHAIN_FORCE_RECOMPUTE", 0) ? pk::kChainForceRecompute : 0);
   static const int block = env_int("PK_CHAIN_BLOCK", 128);
   const int64_t grid = (B + block - 1) / block;
-  pk::ik_chain_kernel<NJ, NFT><<<(unsigned)grid, block, 0, stream>>>(C, q, targets, v, status, B, flags, n_steps, q_out, peers);
+  // PDL unless the fused peer gather is on (peer_gate and its flag protocol assume full stream
+  // order) or the targets row is longer than the kernel's copy of it
+  if (PK_CHAIN_PDL && peers.n == 0 && C.target_stride <= pk::kChainRowWords<NJ, NFT> &&
+      !g_chain_pdl_rejected.load(std::memory_order_relaxed)) {
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3((unsigned)grid);
+    cfg.blockDim = dim3(block);
+    cfg.stream = stream;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[0].val.programmaticStreamSerializationAllowed = 1;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+    if (cudaLaunchKernelEx(&cfg, pk::ik_chain_kernel<NJ, NFT, true>, C, q, targets, v, status, B, flags, n_steps, q_out,
+                           peers) == cudaSuccess) {
+      g_launches.fetch_add(1);
+      return 0;
+    }
+    // a driver or capture mode that rejects the attribute: plain launches from now on
+    cudaGetLastError();
+    g_chain_pdl_rejected.store(true, std::memory_order_relaxed);
+  }
+  pk::ik_chain_kernel<NJ, NFT, false><<<(unsigned)grid, block, 0, stream>>>(C, q, targets, v, status, B, flags, n_steps,
+                                                                          q_out, peers);
   g_launches.fetch_add(1);
   PK_CUDA(cudaGetLastError());
   return 0;

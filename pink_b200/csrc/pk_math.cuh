@@ -114,13 +114,14 @@ PK_HD SE3f load_se3(const float* t) {  // 12 floats, row-major [R | p]
   T.R.m[6] = t[8]; T.R.m[7] = t[9]; T.R.m[8] = t[10]; T.p.z = t[11];
   return T;
 }
-// 12 floats from global memory; `vec4`: the address is 16-byte aligned (three 128-bit
-// read-only loads instead of twelve scalar ones)
+// 12 floats; `vec4`: the address is 16-byte aligned (three 128-bit read-only loads instead
+// of twelve scalar ones when it is in global memory)
 PK_HD SE3f load_se3_vec4(const float* t, bool vec4) {
 #if defined(__CUDA_ARCH__)
   // the caller's `vec4` covers stride and offsets; the base pointer is checked here (a
-  // sliced tensor may start anywhere)
-  if (vec4 && (reinterpret_cast<uintptr_t>(t) & 15u) == 0u) {
+  // sliced tensor may start anywhere).  __ldg only reads global memory: a row the chain
+  // kernel copied to local memory takes the plain loads (resolved at compile time).
+  if (vec4 && __isGlobal(t) && (reinterpret_cast<uintptr_t>(t) & 15u) == 0u) {
     const float4 a = __ldg(reinterpret_cast<const float4*>(t));
     const float4 b = __ldg(reinterpret_cast<const float4*>(t) + 1);
     const float4 c = __ldg(reinterpret_cast<const float4*>(t) + 2);

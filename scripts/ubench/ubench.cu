@@ -2,7 +2,11 @@
 //   1. issue rate of FFMA per SM, ILP 1..8;
 //   2. period of back-to-back kernel nodes in a CUDA graph (empty kernel, and a kernel of
 //      512 CTAs x 128 threads that spins ~5 us), i.e. the launch overhead a 10 us kernel pays;
-//   3. the same with programmatic dependent launch edges.
+//   3. the same with programmatic dependent launch edges (wait at the top: hides launch latency only);
+//   4. a kernel whose CTAs have uneven durations (one in five spins three times as long, like the
+//      chain kernel's Cholesky-round tail), plain and with PDL as the chain kernel uses it:
+//      signal dependents at the top, wait just before the store, so that the next launch
+//      fills the slots the short CTAs free.
 // Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o scripts/ubench/ubench scripts/ubench/ubench.cu
 #include <cstdio>
 #include <cuda_runtime.h>
@@ -37,6 +41,15 @@ __global__ void spin_kernel_pdl(long long cycles, float* sink) {
   while (clock64() - t0 < cycles) {}
   asm volatile("griddepcontrol.launch_dependents;");
   if (sink && threadIdx.x == 0 && blockIdx.x == 0) sink[0] = 1.f;
+}
+
+__global__ void spin_uneven_kernel(long long cycles, float* sink, int pdl) {
+  if (pdl) asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+  const long long n = (blockIdx.x % 5 == 0) ? 3 * cycles : cycles;
+  const long long t0 = clock64();
+  while (clock64() - t0 < n) {}
+  if (pdl) asm volatile("griddepcontrol.wait;" ::: "memory");
+  if (threadIdx.x == 0) sink[blockIdx.x] = 1.f;
 }
 
 template <class F>
@@ -79,13 +92,14 @@ int main() {
   // graph of N kernel nodes: period per node
   cudaStream_t s; CK(cudaStreamCreate(&s));
   const int N = 200;
-  for (int variant = 0; variant < 4; ++variant) {
+  for (int variant = 0; variant < 6; ++variant) {
     cudaGraph_t g; cudaGraphExec_t ge;
     CK(cudaStreamBeginCapture(s, cudaStreamCaptureModeThreadLocal));
     for (int i = 0; i < N; ++i) {
       if (variant == 0) empty_kernel<<<1, 32, 0, s>>>();
       else if (variant == 1) empty_kernel<<<512, 128, 0, s>>>();
       else if (variant == 2) spin_kernel<<<512, 128, 0, s>>>(10000, out);
+      else if (variant == 4) spin_uneven_kernel<<<512, 128, 0, s>>>(10000, out, 0);
       else {
         cudaLaunchConfig_t cfg = {};
         cfg.gridDim = dim3(512); cfg.blockDim = dim3(128); cfg.stream = s;
@@ -93,7 +107,8 @@ int main() {
         at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
         at[0].val.programmaticStreamSerializationAllowed = 1;
         cfg.attrs = at; cfg.numAttrs = 1;
-        CK(cudaLaunchKernelEx(&cfg, spin_kernel_pdl, (long long)10000, out));
+        if (variant == 3) CK(cudaLaunchKernelEx(&cfg, spin_kernel_pdl, (long long)10000, out));
+        else CK(cudaLaunchKernelEx(&cfg, spin_uneven_kernel, (long long)10000, out, 1));
       }
     }
     CK(cudaStreamEndCapture(s, &g));
@@ -105,7 +120,10 @@ int main() {
       cudaEventRecord(e0, s); cudaGraphLaunch(ge, s); cudaEventRecord(e1, s); cudaEventSynchronize(e1);
       float ms; cudaEventElapsedTime(&ms, e0, e1); if (ms < best) best = ms;
     }
-    const char* names[] = {"empty <<<1,32>>>", "empty <<<512,128>>>", "spin 10000 clk <<<512,128>>>", "spin 10000 clk <<<512,128>>> + PDL"};
+    const char* names[] = {"empty <<<1,32>>>", "empty <<<512,128>>>", "spin 10000 clk <<<512,128>>>",
+                           "spin 10000 clk <<<512,128>>> + PDL (wait at the top)",
+                           "uneven spin 10000 / 30000 clk <<<512,128>>>",
+                           "uneven spin 10000 / 30000 clk <<<512,128>>> + PDL (signal at the top, wait before the store)"};
     printf("graph of %d nodes, %s: %.2f us per node\n", N, names[variant], best * 1e3 / N);
     cudaGraphExecDestroy(ge); cudaGraphDestroy(g);
   }
