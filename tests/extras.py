@@ -127,6 +127,79 @@ def ur5_extras(B, seed=3, active=True):
                          [lc], [olc], dt, workloads.UR5_DT and 1e-12, cm, safety_break=True)
 
 
+def as_extra(sc):
+    """A helpers.Scenario (tasks and limits only) in ExtraScenario form."""
+    olimits = None if sc.oracle_limits is None else list(sc.oracle_limits)
+    return ExtraScenario(sc.model, sc.table, sc.q32, list(sc.tasks), list(sc.oracle_tasks), list(sc.limits), olimits,
+                         [], [], [], [], sc.dt, sc.damping, safety_break=sc.safety_break)
+
+
+def with_shared_acceleration_limit(sc, a_max, seed=13):
+    """Adds an AccelerationLimit fed ONE previous velocity ``[nv]`` shared by every instance,
+    as the reference's unbatched usage does.  A shared non-zero previous displacement is not a
+    per-instance box, so the chain and tree kernels decline the problem and the general path
+    (ik_generic_kernel) solves it."""
+    rng = np.random.default_rng(seed)
+    nv = sc.table.nv
+    v_prev = (rng.normal(size=nv) * 0.3).astype(np.float32)
+    acc = AccelerationLimit(sc.model, a_max)
+    acc.set_last_integration(v_prev, sc.dt)
+    # the oracle takes dq_prev per instance: the shared row broadcast to [B, nv]
+    dq_prev = (torch.as_tensor(v_prev) * sc.dt).numpy().astype(np.float64)[None].repeat(sc.B, axis=0)
+    sc.limits = [lim for lim in sc.limits if not isinstance(lim, AccelerationLimit)] + [acc]
+    olimits = [("configuration", 0.5), ("velocity", None)] if sc.olimits is None else \
+        [lim for lim in sc.olimits if lim[0] != "acceleration"]
+    sc.olimits = olimits + [("acceleration", np.asarray(a_max, dtype=np.float64), dq_prev)]
+    return sc
+
+
+def tree_rows_scenario(nj, B, free_flyer=False, frames=(), com=False, linear_rows=(), limits=True, seed=11):
+    """Random tree (helpers.random_tree_model) with a task set of an exact task-row count K.
+
+    ``frames`` lists ``(tip, position_cost, orientation_cost)`` on the tip frames (a zero cost
+    component drops its row), ``com`` adds a CoM task (3 rows) and every entry of
+    ``linear_rows`` a LinearHolonomicTask with that many rows (1..6) on random joint
+    coordinates.  A posture task (no task rows) keeps H well conditioned; ``limits=False``
+    leaves the box empty, so that every factorisation has all nv columns free."""
+    rng = np.random.default_rng(seed)
+    model = helpers.random_tree_model(nj, rng, free_flyer)
+    table = model.table()
+    q = workloads.sample_configurations(table, B, rng)
+    qt = workloads.perturb_configurations(table, q, rng, sigma=0.15)
+    tasks, otasks = [], []
+    for tip, pc, oc in frames:
+        t, o = _frame_task(table, f"tip{tip}", qt, pc, oc, lm_damping=0.02)
+        tasks.append(t)
+        otasks.append(o)
+    if com:
+        c = okin.center_of_mass(table, okin.forward_kinematics(table, qt)).astype(np.float32)
+        ct = ComTask(cost=2.0)
+        ct.set_target(torch.as_tensor(c))
+        tasks.append(ct)
+        otasks.append({"type": "com", "cost": np.full(3, 2.0), "gain": 1.0, "lm_damping": 0.0,
+                       "target": c.astype(np.float64)})
+    rv = 6 if free_flyer else 0
+    for rows in linear_rows:
+        A = np.zeros((rows, table.nv))
+        for r in range(rows):
+            cols = rv + rng.choice(table.nv - rv, size=3, replace=False)
+            A[r, cols] = rng.uniform(-1.0, 1.0, size=3)
+        b = rng.uniform(-0.05, 0.05, size=rows)
+        tasks.append(LinearHolonomicTask(A, b, None, cost=[0.5] * rows, gain=0.5))
+        otasks.append({"type": "linear", "A": A, "b": b, "q0": None, "cost": np.full(rows, 0.5), "gain": 0.5,
+                       "lm_damping": 0.0})
+    q_ref = q[0].copy()
+    pt = PostureTask(cost=0.1)
+    pt.set_target(q_ref)
+    tasks.append(pt)
+    otasks.append({"type": "posture", "cost": 0.1, "gain": 1.0, "lm_damping": 0.0, "target": q_ref})
+    if limits:
+        lims, olims = [ConfigurationLimit(model), VelocityLimit(model)], [("configuration", 0.5), ("velocity", None)]
+    else:
+        lims, olims = [], []
+    return ExtraScenario(model, table, q, tasks, otasks, lims, olims, [], [], [], [], 1.0 / 100.0, 1e-6)
+
+
 def g1_extras(B, seed=5, floating_base_limit=True):
     """G1-class humanoid (config 4 of BASELINE.json): CoM + feet + pelvis + wrist
     tasks, posture, a knee coupling task, default limits + floating-base velocity

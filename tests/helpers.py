@@ -220,7 +220,11 @@ def random_chain_model(nj, rng, prismatic=(), name="chain"):
     return model
 
 
-def chain_scenario(nj, B, seed=1, prismatic=(), two_tasks=False, shared_target=False):
+def chain_scenario(nj, B, seed=1, prismatic=(), two_tasks=False, shared_target=False, frame_tasks=True,
+                   posture_per_instance=False):
+    """Frame task(s) on the random chain plus a posture task.  ``frame_tasks=False`` leaves the
+    posture task alone (no frame task); ``posture_per_instance`` gives it a target row per
+    instance (a targets row of 12 NFT + NJ floats)."""
     rng = np.random.default_rng(seed)
     model = random_chain_model(nj, rng, prismatic)
     table = model.table()
@@ -228,6 +232,7 @@ def chain_scenario(nj, B, seed=1, prismatic=(), two_tasks=False, shared_target=F
     qt = workloads.perturb_configurations(table, q, rng, sigma=0.2)
     tasks, otasks = [], []
     frames = [("tool", 1.0, 0.7)] + ([("elbow", [0.5, 0.0, 2.0], 0.3)] if two_tasks else [])
+    frames = frames if frame_tasks else []
     for frame, pc, oc in frames:
         T = frame_targets(table, qt, frame)
         t = FrameTask(frame, position_cost=pc, orientation_cost=oc, lm_damping=0.1, gain=0.9)
@@ -242,9 +247,13 @@ def chain_scenario(nj, B, seed=1, prismatic=(), two_tasks=False, shared_target=F
         T64 = T.astype(np.float64)
         otasks.append({"type": "frame", "frame": table.frame_names.index(frame), "cost": np.array(t.cost),
                        "gain": 0.9, "lm_damping": 0.1, "target": (T64[:, :, :3], T64[:, :, 3])})
-    q_ref = np.zeros(nj)
+    if posture_per_instance:
+        q_ref32 = workloads.perturb_configurations(table, q, rng, sigma=0.3).astype(np.float32)
+        q_ref = q_ref32.astype(np.float64)
+    else:
+        q_ref32 = q_ref = np.zeros(nj)
     pt = PostureTask(cost=0.05, gain=0.5)
-    pt.set_target(q_ref)
+    pt.set_target(torch.as_tensor(q_ref32) if posture_per_instance else q_ref)
     tasks.append(pt)
     otasks.append({"type": "posture", "cost": 0.05, "gain": 0.5, "lm_damping": 0.0, "target": q_ref})
 

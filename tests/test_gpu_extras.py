@@ -182,9 +182,9 @@ def test_config4_full_batch_feasibility_and_sample_parity(floating_base_limit):
     """BASELINE config 4 at full size (B = 16384, G1-class + sphere self-collision
     barrier): every velocity flagged OK satisfies the dense rows and the box of its own
     QP (rows exported by pk_constraint_rows_batched), infeasible instances are flagged with
-    zero velocity, and a random sample matches the oracle.  Without the floating-base
-    limit the warp-cooperative kernel runs (dual QP in shared memory), with it the
-    general path."""
+    zero velocity, and a random sample matches the oracle.  Both variants run on the
+    warp-cooperative kernel (dual QP in shared memory); the floating-base limit adds its
+    rows to that dual QP.  The general path's solve is tested in test_gpu_kernel_paths.py."""
     sc = extras.g1_extras(16384, floating_base_limit=floating_base_limit)
     v, st = _solve(sc)
     ok = st == 0
