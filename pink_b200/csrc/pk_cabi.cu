@@ -17,7 +17,7 @@
 #include "pk_chain.cuh"
 #include "pk_coop_kernel.cuh"
 #include "pk_generic.cuh"
-#include "pk_marshal.hpp"
+#include "pk_select.hpp"
 
 namespace {
 
@@ -324,9 +324,6 @@ __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;"
 
 // flags bit: after the wait, recompute every instance as if its inputs had changed (tests)
 constexpr int kChainForceRecompute = 4;
-// longest targets row the PDL instantiation copies: frame targets, posture and dq_prev
-template <int NJ, int NFT>
-constexpr int kChainRowWords = 12 * NFT + 2 * NJ;
 
 template <bool CG>
 __device__ __forceinline__ float4 chain_ld4(const float* p) {
@@ -385,9 +382,9 @@ __global__ void __launch_bounds__(128, 4)
   }
   const float* grow = targets + i * (int64_t)P.target_stride;
   const float* trow = grow;
-  // PDL: [targets row (target_stride <= kChainRowWords words) | q row] as the steps use them
-  __align__(16) float used[PDL ? kChainRowWords<NJ, NFT> + NJ : 1];
-  float* const used_q = used + (PDL ? kChainRowWords<NJ, NFT> : 0);
+  // PDL: [targets row (target_stride <= chain_row_words words) | q row] as the steps use them
+  __align__(16) float used[PDL ? chain_row_words(NJ, NFT) + NJ : 1];
+  float* const used_q = used + (PDL ? chain_row_words(NJ, NFT) : 0);
   const bool v4 = P.target_vec4 && (reinterpret_cast<uintptr_t>(grow) & 15u) == 0u;
   if constexpr (PDL) {
     chain_copy_row<false>(used, grow, P.target_stride, v4);
@@ -488,55 +485,12 @@ __global__ void __launch_bounds__(128, 4)
 }
 
 // General path: one instance per thread, per-thread arrays in local memory.
-struct GenericArgs {
-  const float* q;
-  const float* targets;
-  float* v;
-  int32_t* status;
-  float* H;
-  float* c;
-  float* h;
-  float* e;
-  float* J;
-  int task_index;
-  int task_k;
-  float* oMf;
-  float* com;
-  float* Jf;
-  int jac_frame;
-  float* G;
-  float* hG;
-  float* E;
-  float* f;
-  float* lo;
-  float* hi;
-};
-
 template <int NJMAX, int NVMAX>
 __global__ void __launch_bounds__(64) ik_generic_kernel(const DevModel M, const __grid_constant__ DevProblem P,
                                                         const GenericArgs A, int64_t B) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= B) return;
-  const int nv = M.nv;
-  GenericOut out;
-  out.v = A.v ? A.v + i * nv : nullptr;
-  out.status = A.status ? A.status + i : nullptr;
-  out.H = A.H ? A.H + i * nv * nv : nullptr;
-  out.c = A.c ? A.c + i * nv : nullptr;
-  out.h = A.h ? A.h + i * 4 * nv : nullptr;
-  out.e = A.e ? A.e + i * A.task_k : nullptr;
-  out.J = A.J ? A.J + i * A.task_k * nv : nullptr;
-  out.task_index = A.task_index;
-  out.oMf = A.oMf ? A.oMf + i * M.nframes * 12 : nullptr;
-  out.com = A.com ? A.com + i * 3 : nullptr;
-  out.Jf = A.Jf ? A.Jf + i * 6 * nv : nullptr;
-  out.jac_frame = A.jac_frame;
-  out.G = A.G ? A.G + i * PK_MAX_INEQ_ROWS * nv : nullptr;
-  out.hG = A.hG ? A.hG + i * PK_MAX_INEQ_ROWS : nullptr;
-  out.E = A.E ? A.E + i * PK_MAX_EQ_ROWS * nv : nullptr;
-  out.f = A.f ? A.f + i * PK_MAX_EQ_ROWS : nullptr;
-  out.lo = A.lo ? A.lo + i * nv : nullptr;
-  out.hi = A.hi ? A.hi + i * nv : nullptr;
+  const GenericOut out = generic_out(M, A, i);
   Generic<NJMAX, NVMAX> G;
   G.step(M, P, A.q + i * M.nq, A.targets ? A.targets + i * (int64_t)P.target_stride : nullptr, out);
 }
@@ -668,9 +622,18 @@ int env_int(const char* name, int dflt) {
   return s ? atoi(s) : dflt;
 }
 
+// Epilogue of every kernel launch.
+int launched() {
+  g_launches.fetch_add(1);
+  PK_CUDA(cudaGetLastError());
+  return 0;
+}
+
+const pk::PeerOut kNoPeers{};
+
 template <int NJ, int NFT>
-int launch_chain_nft(const pk::ChainParams<NJ>& C, const float* q, const float* targets, float* v, int32_t* status,
-                     int64_t B, cudaStream_t stream, int n_steps, float* q_out, const pk::PeerOut& peers) {
+int launch_chain(const pk::ChainParams<NJ>& C, bool pdl_row_fits, const float* q, const float* targets, float* v,
+                 int32_t* status, int64_t B, cudaStream_t stream, int n_steps, float* q_out, const pk::PeerOut& peers) {
   // A/B and probe switches (timing experiments; see scripts/ab.sh)
   static const int flags = (env_int("PK_CLOSED_FORM", 1) ? 0 : 1) | (env_int("PK_PROBE_SKIP_ROUNDS", 0) ? 2 : 0) |
                            (env_int("PK_CHAIN_FORCE_RECOMPUTE", 0) ? pk::kChainForceRecompute : 0);
@@ -678,8 +641,7 @@ int launch_chain_nft(const pk::ChainParams<NJ>& C, const float* q, const float* 
   const int64_t grid = (B + block - 1) / block;
   // PDL unless the fused peer gather is on (peer_gate and its flag protocol assume full stream
   // order) or the targets row is longer than the kernel's copy of it
-  if (PK_CHAIN_PDL && peers.n == 0 && C.target_stride <= pk::kChainRowWords<NJ, NFT> &&
-      !g_chain_pdl_rejected.load(std::memory_order_relaxed)) {
+  if (PK_CHAIN_PDL && peers.n == 0 && pdl_row_fits && !g_chain_pdl_rejected.load(std::memory_order_relaxed)) {
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3((unsigned)grid);
     cfg.blockDim = dim3(block);
@@ -690,52 +652,57 @@ int launch_chain_nft(const pk::ChainParams<NJ>& C, const float* q, const float* 
     cfg.attrs = attr;
     cfg.numAttrs = 1;
     if (cudaLaunchKernelEx(&cfg, pk::ik_chain_kernel<NJ, NFT, true>, C, q, targets, v, status, B, flags, n_steps, q_out,
-                           peers) == cudaSuccess) {
-      g_launches.fetch_add(1);
-      return 0;
-    }
+                           peers) == cudaSuccess)
+      return launched();
     // a driver or capture mode that rejects the attribute: plain launches from now on
     cudaGetLastError();
     g_chain_pdl_rejected.store(true, std::memory_order_relaxed);
   }
   pk::ik_chain_kernel<NJ, NFT, false><<<(unsigned)grid, block, 0, stream>>>(C, q, targets, v, status, B, flags, n_steps,
                                                                           q_out, peers);
-  g_launches.fetch_add(1);
-  PK_CUDA(cudaGetLastError());
-  return 0;
+  return launched();
 }
 
-template <int NJ>
-int launch_chain(const pk::ChainParams<NJ>& C, const float* q, const float* targets, float* v, int32_t* status,
-                 int64_t B, cudaStream_t stream, int n_steps = 1, float* q_out = nullptr,
-                 const pk::PeerOut* peers = nullptr) {
-  static const pk::PeerOut none{};
-  const pk::PeerOut& po = peers ? *peers : none;
-  switch (C.n_frame_tasks) {
-    case 0: return launch_chain_nft<NJ, 0>(C, q, targets, v, status, B, stream, n_steps, q_out, po);
-    case 1: return launch_chain_nft<NJ, 1>(C, q, targets, v, status, B, stream, n_steps, q_out, po);
-    default: return launch_chain_nft<NJ, 2>(C, q, targets, v, status, B, stream, n_steps, q_out, po);
-  }
-}
-
-int launch_generic(const PkModel* m, const pk::DevProblem& P, const pk::GenericArgs& A, int64_t B,
+// size_class: pk::generic_size_class of the model
+int launch_generic(const PkModel* m, int size_class, const pk::DevProblem& P, const pk::GenericArgs& A, int64_t B,
                    cudaStream_t stream) {
   const int block = 64;
   const int64_t grid = (B + block - 1) / block;
-  if (m->nv <= 8 && m->njoints <= 8)
-    pk::ik_generic_kernel<8, 8><<<(unsigned)grid, block, 0, stream>>>(m->dev, P, A, B);
-  else if (m->nv <= 36 && m->njoints <= 30)
-    pk::ik_generic_kernel<30, 36><<<(unsigned)grid, block, 0, stream>>>(m->dev, P, A, B);
-  else
-    pk::ik_generic_kernel<PK_MAX_JOINTS, PK_MAX_NV><<<(unsigned)grid, block, 0, stream>>>(m->dev, P, A, B);
-  g_launches.fetch_add(1);
-  PK_CUDA(cudaGetLastError());
-  return 0;
+  pk::with_generic(size_class, [&](auto nj, auto nv) {
+    pk::ik_generic_kernel<decltype(nj)::value, decltype(nv)::value><<<(unsigned)grid, block, 0, stream>>>(m->dev, P, A, B);
+  });
+  return launched();
+}
+
+// Dynamic shared memory a kernel has been granted, per device ordinal: the opt-in is per device,
+// and the entry points may run on several host threads.
+struct SmemGrant {
+  std::mutex mu;
+  size_t bytes[64] = {};
+};
+SmemGrant g_tree_smem, g_tree_rollout_smem;
+
+// A tree kernel: one instance per warp, `plan.words` floats of dynamic shared memory per warp.
+template <class... Params, class... Args>
+int launch_tree(void (*kernel)(Params...), SmemGrant& grant, const PkModel* m, const pk::TreePlan& plan, int64_t B,
+                cudaStream_t stream, const Args&... args) {
+  const size_t smem = (size_t)plan.words * 4 * pk::kTreeWarpsPerBlock;
+  {
+    std::lock_guard<std::mutex> lock(grant.mu);
+    const int dev = (m->device >= 0 && m->device < 64) ? m->device : 0;
+    if (smem > grant.bytes[dev] || m->device >= 64) {
+      PK_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+      grant.bytes[dev] = smem;
+    }
+  }
+  const int64_t grid = (B + pk::kTreeWarpsPerBlock - 1) / pk::kTreeWarpsPerBlock;
+  kernel<<<(unsigned)grid, 32 * pk::kTreeWarpsPerBlock, smem, stream>>>(args...);
+  return launched();
 }
 
 }  // namespace
 
-// A validated problem with its kernel parameter blocks precomputed, so that the
+// A validated problem with its kernel selection and parameter blocks precomputed, so that the
 // per-call host cost is one kernel launch.
 struct PkProblem {
   pk::DevProblem P;
@@ -749,34 +716,13 @@ struct PkProblem {
     if (ext_async) cudaFreeAsync(dev_ext, ext_stream);
     else cudaFree(dev_ext);
   }
-  bool chain = false;
-  bool tree = false;
-  pk::TreePlan plan;
-  int nj = 0;
+  pk::Selection sel;
   alignas(16) unsigned char chain_params[sizeof(pk::ChainParams<7>)];
-  // parameter blocks of the sub-warp chain kernel, one per lanes-per-instance variant
-  // (index log2 L); the padding joints depend on L
-  alignas(16) unsigned char coop_params[4][sizeof(pk::CoopParams<8>)];
+  // parameter block of the sub-warp chain kernel's variant sel.lanes (the padding joints depend on it)
+  alignas(16) unsigned char coop_params[sizeof(pk::CoopParams<8>)];
 };
 
 namespace {
-
-template <int NJ, int L>
-void fill_coop(const PkModel* m, PkProblem* pr, const pk::DevExtras* X, int slot) {
-  constexpr int NJP = pk::CoopStep<NJ, 1, L>::NJP;
-  static_assert(sizeof(pk::CoopParams<NJP>) <= sizeof(pr->coop_params[0]), "parameter block too small");
-  pk::make_coop_params<NJ, L>(m->hm, pr->P, reinterpret_cast<pk::CoopParams<NJP>*>(pr->coop_params[slot]), X);
-}
-
-template <int NJ>
-void fill_chain(const PkModel* m, PkProblem* pr, const pk::DevExtras* X) {
-  static_assert(sizeof(pk::ChainParams<NJ>) <= sizeof(pr->chain_params), "parameter block too small");
-  pk::make_chain_params<NJ>(m->hm, pr->P, reinterpret_cast<pk::ChainParams<NJ>*>(pr->chain_params), X);
-  fill_coop<NJ, 1>(m, pr, X, 0);
-  fill_coop<NJ, 2>(m, pr, X, 1);
-  fill_coop<NJ, 4>(m, pr, X, 2);
-  fill_coop<NJ, 8>(m, pr, X, 3);
-}
 
 // Device image of the optional problem parts: [DevExtras | extra | pairs] in one buffer.
 // With `stream` the allocation and copies are stream-ordered (temporary problems of the
@@ -814,112 +760,73 @@ int prepare_problem(const PkModel* m, const PkProblemDesc* desc, PkProblem* pr, 
     pr->ext_stream = stream;
     pr->P.ext = reinterpret_cast<const pk::DevExtras*>(pr->dev_ext);
   }
-  static const int force_generic = env_int("PK_FORCE_GENERIC", 0);
-  pr->chain = !force_generic && pk::chain_eligible(m->hm, pr->P, hx.present && !hx.box_only());
-  pr->nj = m->njoints;
-  static const int use_tree = env_int("PK_TREE", 1);
-  bool tree_ok = false;
-  pr->plan = pk::make_tree_plan(m->hm, pr->P, &tree_ok, hx.present ? &hx.X : nullptr);
-  pr->tree = !force_generic && use_tree && !pr->chain && tree_ok;
-  if (pr->chain) {
-    switch (m->njoints) {
-      case 2: fill_chain<2>(m, pr, hx.present ? &hx.X : nullptr); break;
-      case 3: fill_chain<3>(m, pr, hx.present ? &hx.X : nullptr); break;
-      case 4: fill_chain<4>(m, pr, hx.present ? &hx.X : nullptr); break;
-      case 5: fill_chain<5>(m, pr, hx.present ? &hx.X : nullptr); break;
-      case 6: fill_chain<6>(m, pr, hx.present ? &hx.X : nullptr); break;
-      case 7: fill_chain<7>(m, pr, hx.present ? &hx.X : nullptr); break;
-      default: pr->chain = false;
-    }
-  }
-  return 0;
-}
-
-template <int NJ, int NFT, int L>
-int launch_coop_nft(const PkProblem& pr, int slot, const float* q, const float* targets, float* v, int32_t* status,
-                    int64_t B, cudaStream_t stream, int n_steps, float* q_out) {
-  using Step = pk::CoopStep<NJ, NFT, L>;
-  const auto& C = *reinterpret_cast<const pk::CoopParams<Step::NJP>*>(pr.coop_params[slot]);
-  const int64_t grid = (B * L + pk::kCoopThreads - 1) / pk::kCoopThreads;
-  pk::ik_coop_kernel<NJ, NFT, L><<<(unsigned)grid, pk::kCoopThreads, 0, stream>>>(C, q, targets, v, status, B, n_steps, q_out);
-  g_launches.fetch_add(1);
-  PK_CUDA(cudaGetLastError());
-  return 0;
-}
-
-template <int NJ, int L>
-int launch_coop(const PkProblem& pr, int slot, const float* q, const float* targets, float* v, int32_t* status,
-                int64_t B, cudaStream_t stream, int n_steps, float* q_out) {
-  const int nft = reinterpret_cast<const pk::CoopParams<pk::CoopStep<NJ, 1, L>::NJP>*>(pr.coop_params[slot])->n_frame_tasks;
-  switch (nft) {
-    case 0: return launch_coop_nft<NJ, 0, L>(pr, slot, q, targets, v, status, B, stream, n_steps, q_out);
-    case 1: return launch_coop_nft<NJ, 1, L>(pr, slot, q, targets, v, status, B, stream, n_steps, q_out);
-    default: return launch_coop_nft<NJ, 2, L>(pr, slot, q, targets, v, status, B, stream, n_steps, q_out);
-  }
-}
-
-template <int NJ>
-int launch_chain_prepared(const PkProblem& pr, const float* q, const float* targets, float* v, int32_t* status,
-                          int64_t B, cudaStream_t stream, int n_steps = 1, float* q_out = nullptr,
-                          const pk::PeerOut* peers = nullptr) {
   // PK_CHAIN_LANES: 0 = round-1 kernel (one instance per thread, pk_chain.cuh); 1 / 2 / 4 / 8 =
-  // sub-warp kernel (pk_coop.cuh) with that many lanes per instance (4 and 8: UR5-class study
-  // variants, 6 joints + 1 frame task only)
-  static const int lanes_env = env_int("PK_CHAIN_LANES", 0);
-  const int lanes = peers ? 0 : lanes_env;  // the fused gather epilogue lives in the thread-per-instance kernel
-  if (lanes == 1) return launch_coop<NJ, 1>(pr, 0, q, targets, v, status, B, stream, n_steps, q_out);
-  if (lanes == 2) return launch_coop<NJ, 2>(pr, 1, q, targets, v, status, B, stream, n_steps, q_out);
-  if constexpr (NJ == 6) {
-    const int nft = reinterpret_cast<const pk::ChainParams<NJ>*>(pr.chain_params)->n_frame_tasks;
-    if (lanes == 4 && nft == 1) return launch_coop_nft<NJ, 1, 4>(pr, 2, q, targets, v, status, B, stream, n_steps, q_out);
-    if (lanes == 8 && nft == 1) return launch_coop_nft<NJ, 1, 8>(pr, 3, q, targets, v, status, B, stream, n_steps, q_out);
-  }
-  return launch_chain<NJ>(*reinterpret_cast<const pk::ChainParams<NJ>*>(pr.chain_params), q, targets, v, status, B,
-                          stream, n_steps, q_out, peers);
+  // sub-warp kernel (pk_coop.cuh) with that many lanes per instance
+  static const pk::SelectOptions opts = [] {
+    pk::SelectOptions o;
+    o.use_chain = !env_int("PK_FORCE_GENERIC", 0);
+    o.use_tree = o.use_chain && env_int("PK_TREE", 1);
+    o.chain_lanes = env_int("PK_CHAIN_LANES", 0);
+    return o;
+  }();
+  const pk::Selection& s = pr->sel = pk::select_kernel(m->hm, pr->P, hx, opts);
+  if (s.path != pk::kPathChain) return 0;
+  const pk::DevExtras* X = hx.present ? &hx.X : nullptr;
+  pk::with_nj(s.nj, [&](auto nj) {
+    constexpr int NJ = decltype(nj)::value;
+    static_assert(sizeof(pk::ChainParams<NJ>) <= sizeof(pr->chain_params), "parameter block too small");
+    pk::make_chain_params<NJ>(m->hm, pr->P, reinterpret_cast<pk::ChainParams<NJ>*>(pr->chain_params), X);
+    if (!s.lanes) return;
+    pk::with_nft(s.nft, [&](auto nft) {
+      pk::with_lanes<NJ, decltype(nft)::value>(s.lanes, [&](auto lanes) {
+        constexpr int L = decltype(lanes)::value;
+        using Params = pk::CoopParams<pk::CoopStep<NJ, decltype(nft)::value, L>::NJP>;
+        static_assert(sizeof(Params) <= sizeof(pr->coop_params), "parameter block too small");
+        pk::make_coop_params<NJ, L>(m->hm, pr->P, reinterpret_cast<Params*>(pr->coop_params), X);
+      });
+    });
+  });
+  return 0;
+}
+
+// The chain kernels of a prepared chain problem; n_steps > 1 or q_out: closed-loop rollout.
+// `peers`: the fused gather epilogue, which lives in the thread-per-instance kernel.
+int launch_chain_prepared(const PkProblem& pr, const float* q, const float* targets, float* v, int32_t* status,
+                          int64_t B, cudaStream_t stream, int n_steps, float* q_out, const pk::PeerOut* peers) {
+  return pk::with_nj(pr.sel.nj, [&](auto nj) {
+    constexpr int NJ = decltype(nj)::value;
+    return pk::with_nft(pr.sel.nft, [&](auto nft) {
+      constexpr int NFT = decltype(nft)::value;
+      if (pr.sel.lanes && !peers) {
+        return pk::with_lanes<NJ, NFT>(pr.sel.lanes, [&](auto lanes) {
+          constexpr int L = decltype(lanes)::value;
+          const auto& C = *reinterpret_cast<const pk::CoopParams<pk::CoopStep<NJ, NFT, L>::NJP>*>(pr.coop_params);
+          const int64_t grid = (B * L + pk::kCoopThreads - 1) / pk::kCoopThreads;
+          pk::ik_coop_kernel<NJ, NFT, L>
+              <<<(unsigned)grid, pk::kCoopThreads, 0, stream>>>(C, q, targets, v, status, B, n_steps, q_out);
+          return launched();
+        });
+      }
+      return launch_chain<NJ, NFT>(*reinterpret_cast<const pk::ChainParams<NJ>*>(pr.chain_params), pr.sel.pdl_row_fits,
+                                   q, targets, v, status, B, stream, n_steps, q_out, peers ? *peers : kNoPeers);
+    });
+  });
 }
 
 int solve_device(const PkModel* m, const PkProblem& pr, const float* q, const float* targets, float* v,
                  int32_t* status, int64_t B, cudaStream_t stream) {
   if (B == 0) return 0;
-  if (pr.chain) {
-    switch (pr.nj) {
-      case 2: return launch_chain_prepared<2>(pr, q, targets, v, status, B, stream);
-      case 3: return launch_chain_prepared<3>(pr, q, targets, v, status, B, stream);
-      case 4: return launch_chain_prepared<4>(pr, q, targets, v, status, B, stream);
-      case 5: return launch_chain_prepared<5>(pr, q, targets, v, status, B, stream);
-      case 6: return launch_chain_prepared<6>(pr, q, targets, v, status, B, stream);
-      case 7: return launch_chain_prepared<7>(pr, q, targets, v, status, B, stream);
-      default: break;
-    }
-  }
-  if (pr.tree) {
-    const size_t smem = (size_t)pr.plan.words * 4 * pk::kTreeWarpsPerBlock;
-    // the opt-in is per device (and this entry point may run on several host threads): keep
-    // the size granted so far per device ordinal, under a lock
-    {
-      static std::mutex cfg_mu;
-      static size_t configured[64] = {};
-      std::lock_guard<std::mutex> lock(cfg_mu);
-      const int dev = (m->device >= 0 && m->device < 64) ? m->device : 0;
-      if (smem > configured[dev] || m->device >= 64) {
-        PK_CUDA(cudaFuncSetAttribute(pk::ik_tree_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        configured[dev] = smem;
-      }
-    }
-    const int64_t grid = (B + pk::kTreeWarpsPerBlock - 1) / pk::kTreeWarpsPerBlock;
-    pk::ik_tree_kernel<<<(unsigned)grid, 32 * pk::kTreeWarpsPerBlock, smem, stream>>>(m->dev, pr.P, pr.plan, q, targets, v,
-                                                                                      status, B);
-    g_launches.fetch_add(1);
-    PK_CUDA(cudaGetLastError());
-    return 0;
-  }
+  if (pr.sel.path == pk::kPathChain) return launch_chain_prepared(pr, q, targets, v, status, B, stream, 1, nullptr, nullptr);
+  if (pr.sel.path == pk::kPathTree)
+    return launch_tree(pk::ik_tree_kernel, g_tree_smem, m, pr.sel.plan, B, stream, m->dev, pr.P, pr.sel.plan, q,
+                       targets, v, status, B);
   pk::GenericArgs A{};
   A.q = q;
   A.targets = targets;
   A.v = v;
   A.status = status;
   A.task_index = -1;
-  return launch_generic(m, pr.P, A, B, stream);
+  return launch_generic(m, pr.sel.generic_class, pr.P, A, B, stream);
 }
 
 int check_common(const PkModel* m, const void* q, int64_t B) {
@@ -1050,37 +957,18 @@ extern "C" int pk_solve_ik_prepared_gather(const PkModel* m, const PkProblem* pr
   cudaStream_t stream = (cudaStream_t)stream_;
   pk::PeerOut po;
   if (fill_peer_out(&po, peer_v, n_peers, row_offset, peer_flags, rank, n_buffers)) return 1;
-  bool launched = false;
-  if (pr->chain) {
-    int rc = -1;
-    switch (pr->nj) {
-      case 2: rc = launch_chain_prepared<2>(*pr, q, targets, v, status, B, stream, 1, nullptr, &po); break;
-      case 3: rc = launch_chain_prepared<3>(*pr, q, targets, v, status, B, stream, 1, nullptr, &po); break;
-      case 4: rc = launch_chain_prepared<4>(*pr, q, targets, v, status, B, stream, 1, nullptr, &po); break;
-      case 5: rc = launch_chain_prepared<5>(*pr, q, targets, v, status, B, stream, 1, nullptr, &po); break;
-      case 6: rc = launch_chain_prepared<6>(*pr, q, targets, v, status, B, stream, 1, nullptr, &po); break;
-      case 7: rc = launch_chain_prepared<7>(*pr, q, targets, v, status, B, stream, 1, nullptr, &po); break;
-      default: break;
-    }
-    if (rc > 0) return rc;
-    launched = rc == 0;
-  }
-  if (!launched) {
-    // kernels without the fused epilogue: solve into v, then one scatter kernel
-    if (!v) return fail("this model needs a local v buffer for the gather");
-    if (solve_device(m, *pr, q, targets, v, status, B, stream)) return 1;
-    if (n_peers > 0) {
-      const int64_t n = B * m->nv;
-      const int block = 256;
-      int sms = 0;
-      PK_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, m->device));
-      const int64_t grid = std::min<int64_t>((n + block - 1) / block, (int64_t)sms * 8);
-      pk::peer_scatter_kernel<<<(unsigned)grid, block, 0, stream>>>(v, n, po, m->nv);
-      g_launches.fetch_add(1);
-      PK_CUDA(cudaGetLastError());
-    }
-  }
-  return 0;
+  if (pr->sel.path == pk::kPathChain) return launch_chain_prepared(*pr, q, targets, v, status, B, stream, 1, nullptr, &po);
+  // kernels without the fused epilogue: solve into v, then one scatter kernel
+  if (!v) return fail("this model needs a local v buffer for the gather");
+  if (solve_device(m, *pr, q, targets, v, status, B, stream)) return 1;
+  if (n_peers == 0) return 0;
+  const int64_t n = B * m->nv;
+  const int block = 256;
+  int sms = 0;
+  PK_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, m->device));
+  const int64_t grid = std::min<int64_t>((n + block - 1) / block, (int64_t)sms * 8);
+  pk::peer_scatter_kernel<<<(unsigned)grid, block, 0, stream>>>(v, n, po, m->nv);
+  return launched();
 }
 
 extern "C" int pk_peer_sync(int device, void* const* peer_flags, int32_t n_peers, int32_t rank, int32_t post,
@@ -1108,37 +996,11 @@ extern "C" int pk_rollout_prepared(const PkModel* m, const PkProblem* pr, const 
   if (B > 0 && pr->P.target_stride > 0 && !targets) return fail("null targets");
   if (B == 0) return 0;
   cudaStream_t stream = (cudaStream_t)stream_;
-  if (pr->chain) {
-    switch (pr->nj) {
-      case 2: return launch_chain_prepared<2>(*pr, q, targets, v, status, B, stream, n_steps, q_out);
-      case 3: return launch_chain_prepared<3>(*pr, q, targets, v, status, B, stream, n_steps, q_out);
-      case 4: return launch_chain_prepared<4>(*pr, q, targets, v, status, B, stream, n_steps, q_out);
-      case 5: return launch_chain_prepared<5>(*pr, q, targets, v, status, B, stream, n_steps, q_out);
-      case 6: return launch_chain_prepared<6>(*pr, q, targets, v, status, B, stream, n_steps, q_out);
-      case 7: return launch_chain_prepared<7>(*pr, q, targets, v, status, B, stream, n_steps, q_out);
-      default: break;
-    }
-  }
-  if (pr->tree) {
-    // joint trees: the whole loop in one launch of the warp kernel
-    const size_t smem = (size_t)pr->plan.words * 4 * pk::kTreeWarpsPerBlock;
-    {
-      static std::mutex cfg_mu;
-      static size_t configured[64] = {};
-      std::lock_guard<std::mutex> lock(cfg_mu);
-      const int dev = (m->device >= 0 && m->device < 64) ? m->device : 0;
-      if (smem > configured[dev] || m->device >= 64) {
-        PK_CUDA(cudaFuncSetAttribute(pk::ik_tree_rollout_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        configured[dev] = smem;
-      }
-    }
-    const int64_t grid = (B + pk::kTreeWarpsPerBlock - 1) / pk::kTreeWarpsPerBlock;
-    pk::ik_tree_rollout_kernel<<<(unsigned)grid, 32 * pk::kTreeWarpsPerBlock, smem, stream>>>(
-        m->dev, pr->P, pr->plan, q, targets, n_steps, q_out, v, status, B);
-    g_launches.fetch_add(1);
-    PK_CUDA(cudaGetLastError());
-    return 0;
-  }
+  if (pr->sel.path == pk::kPathChain)
+    return launch_chain_prepared(*pr, q, targets, v, status, B, stream, n_steps, q_out, nullptr);
+  if (pr->sel.path == pk::kPathTree)  // joint trees: the whole loop in one launch of the warp kernel
+    return launch_tree(pk::ik_tree_rollout_kernel, g_tree_rollout_smem, m, pr->sel.plan, B, stream, m->dev, pr->P,
+                       pr->sel.plan, q, targets, n_steps, q_out, v, status, B);
   // other models: the same closed loop as separate launches (solve, then integrate in place)
   if (q_out != q) PK_CUDA(cudaMemcpyAsync(q_out, q, sizeof(float) * B * m->nq, cudaMemcpyDeviceToDevice, stream));
   for (int s = 0; s < n_steps; ++s) {
@@ -1226,6 +1088,31 @@ static int solve_host_impl(PkModel* m, const PkProblem& pr, const float* q_host,
   int64_t chunk = std::max<int64_t>(1024, chunk_env);
   if ((B + chunk - 1) / chunk > PkModel::kMaxChunks) chunk = (B + PkModel::kMaxChunks - 1) / PkModel::kMaxChunks;
   const int64_t nchunks = (B + chunk - 1) / chunk;
+  // chunk k: rows [k chunk, k chunk + rows(k)) of the call
+  auto rows = [&](int64_t k) { return std::min(chunk, B - k * chunk); };
+  auto upload = [&](int64_t k, cudaStream_t s) {
+    const int64_t b0 = k * chunk;
+    PK_CUDA(cudaMemcpyAsync(S.st_q + b0 * m->nq, q_host + b0 * m->nq, sizeof(float) * rows(k) * m->nq,
+                            cudaMemcpyHostToDevice, s));
+    if (ts > 0)
+      PK_CUDA(cudaMemcpyAsync(S.st_t + b0 * ts, targets_host + b0 * ts, sizeof(float) * rows(k) * ts,
+                              cudaMemcpyHostToDevice, s));
+    return 0;
+  };
+  // v / status of the chunk into v_out / status_out: the staging buffers or the caller's pinned ones
+  auto solve = [&](int64_t k, float* v_out, int32_t* status_out, cudaStream_t s) {
+    const int64_t b0 = k * chunk;
+    return solve_device(m, pr, S.st_q + b0 * m->nq, S.st_t + b0 * ts, v_out + b0 * m->nv,
+                        status_out ? status_out + b0 : nullptr, rows(k), s);
+  };
+  auto download = [&](int64_t k, cudaStream_t s) {
+    const int64_t b0 = k * chunk;
+    PK_CUDA(cudaMemcpyAsync(v_host + b0 * m->nv, S.st_v + b0 * m->nv, sizeof(float) * rows(k) * m->nv,
+                            cudaMemcpyDeviceToHost, s));
+    if (status_host)
+      PK_CUDA(cudaMemcpyAsync(status_host + b0, S.st_s + b0, sizeof(int32_t) * rows(k), cudaMemcpyDeviceToHost, s));
+    return 0;
+  };
   // PK_HOST_DUPLEX=1: chunks round-robin over three internal streams, so that the H2D of
   // chunk k+1, the kernel of chunk k and the D2H of chunk k-1 overlap.  Default (0): the
   // two directions never overlap - all uploads on one stream, each kernel as soon as its
@@ -1240,19 +1127,7 @@ static int solve_host_impl(PkModel* m, const PkProblem& pr, const float* q_host,
     for (int i = 0; i < nstreams; ++i) PK_CUDA(cudaStreamWaitEvent(S.st_streams[i], S.st_fork, 0));
     for (int64_t k = 0; k < nchunks; ++k) {
       cudaStream_t s = S.st_streams[k % nstreams];
-      const int64_t b0 = k * chunk;
-      const int64_t nb = std::min(chunk, B - b0);
-      PK_CUDA(cudaMemcpyAsync(S.st_q + b0 * m->nq, q_host + b0 * m->nq, sizeof(float) * nb * m->nq,
-                              cudaMemcpyHostToDevice, s));
-      if (ts > 0)
-        PK_CUDA(cudaMemcpyAsync(S.st_t + b0 * ts, targets_host + b0 * ts, sizeof(float) * nb * ts,
-                                cudaMemcpyHostToDevice, s));
-      if (solve_device(m, pr, S.st_q + b0 * m->nq, S.st_t + b0 * ts, S.st_v + b0 * m->nv, S.st_s + b0, nb, s))
-        return 1;
-      PK_CUDA(cudaMemcpyAsync(v_host + b0 * m->nv, S.st_v + b0 * m->nv, sizeof(float) * nb * m->nv,
-                              cudaMemcpyDeviceToHost, s));
-      if (status_host)
-        PK_CUDA(cudaMemcpyAsync(status_host + b0, S.st_s + b0, sizeof(int32_t) * nb, cudaMemcpyDeviceToHost, s));
+      if (upload(k, s) || solve(k, S.st_v, S.st_s, s) || download(k, s)) return 1;
     }
     for (int i = 0; i < nstreams; ++i) {
       PK_CUDA(cudaEventRecord(S.st_join[i], S.st_streams[i]));
@@ -1260,8 +1135,11 @@ static int solve_host_impl(PkModel* m, const PkProblem& pr, const float* q_host,
     }
     return 0;
   }
-  // PK_HOST_MODE=2: uploads staged as below, but the kernels write v / status straight into
-  // the caller's pinned host buffers (posted PCIe writes, no download phase)
+  // PK_HOST_MODE=2 ("direct"): uploads staged, but the kernels write v / status straight into
+  // the caller's pinned host buffers (posted PCIe writes, no download phase); staged downloads
+  // when a result buffer is not pinned
+  float* v_dev = nullptr;
+  int32_t* s_dev = nullptr;
   if (host_mode == 2) {
     auto dev_ptr = [](const void* ptr) -> void* {
       if (!ptr) return nullptr;
@@ -1269,39 +1147,13 @@ static int solve_host_impl(PkModel* m, const PkProblem& pr, const float* q_host,
       if (cudaPointerGetAttributes(&a, ptr) != cudaSuccess || a.type != cudaMemoryTypeHost) return nullptr;
       return a.devicePointer;
     };
-    float* v_dev = static_cast<float*>(dev_ptr(v_host));
-    int32_t* s_dev = static_cast<int32_t*>(dev_ptr(status_host));
+    v_dev = static_cast<float*>(dev_ptr(v_host));
+    s_dev = static_cast<int32_t*>(dev_ptr(status_host));
     cudaGetLastError();
-    if (v_dev && (s_dev || !status_host)) {
-      cudaStream_t s_in = S.st_streams[0], s_k = S.st_streams[1];
-      for (int i = 0; i < 2; ++i) PK_CUDA(cudaStreamWaitEvent(S.st_streams[i], S.st_fork, 0));
-      if (S.st_busy) PK_CUDA(cudaStreamWaitEvent(s_in, S.st_join[2], 0));
-      S.st_busy = true;
-      for (int64_t k = 0; k < nchunks; ++k) {
-        if (!S.st_in[k]) {
-          PK_CUDA(cudaEventCreateWithFlags(&S.st_in[k], cudaEventDisableTiming));
-          PK_CUDA(cudaEventCreateWithFlags(&S.st_kern[k], cudaEventDisableTiming));
-        }
-        const int64_t b0 = k * chunk;
-        const int64_t nb = std::min(chunk, B - b0);
-        PK_CUDA(cudaMemcpyAsync(S.st_q + b0 * m->nq, q_host + b0 * m->nq, sizeof(float) * nb * m->nq,
-                                cudaMemcpyHostToDevice, s_in));
-        if (ts > 0)
-          PK_CUDA(cudaMemcpyAsync(S.st_t + b0 * ts, targets_host + b0 * ts, sizeof(float) * nb * ts,
-                                  cudaMemcpyHostToDevice, s_in));
-        PK_CUDA(cudaEventRecord(S.st_in[k], s_in));
-        PK_CUDA(cudaStreamWaitEvent(s_k, S.st_in[k], 0));
-        if (solve_device(m, pr, S.st_q + b0 * m->nq, S.st_t + b0 * ts, v_dev + b0 * m->nv, s_dev ? s_dev + b0 : nullptr,
-                         nb, s_k))
-          return 1;
-      }
-      PK_CUDA(cudaEventRecord(S.st_join[2], s_k));
-      PK_CUDA(cudaStreamWaitEvent(stream, S.st_join[2], 0));
-      return 0;
-    }
   }
+  const bool direct = v_dev && (s_dev || !status_host);
   cudaStream_t s_in = S.st_streams[0], s_k = S.st_streams[1], s_out = S.st_streams[2];
-  for (int i = 0; i < 3; ++i) PK_CUDA(cudaStreamWaitEvent(S.st_streams[i], S.st_fork, 0));
+  for (int i = 0; i < (direct ? 2 : 3); ++i) PK_CUDA(cudaStreamWaitEvent(S.st_streams[i], S.st_fork, 0));
   // calls submitted on different caller streams share the staging buffers: the next upload
   // waits for the previous call's last download (a no-op for calls on one stream)
   if (S.st_busy) PK_CUDA(cudaStreamWaitEvent(s_in, S.st_join[2], 0));
@@ -1311,32 +1163,22 @@ static int solve_host_impl(PkModel* m, const PkProblem& pr, const float* q_host,
       PK_CUDA(cudaEventCreateWithFlags(&S.st_in[k], cudaEventDisableTiming));
       PK_CUDA(cudaEventCreateWithFlags(&S.st_kern[k], cudaEventDisableTiming));
     }
-    const int64_t b0 = k * chunk;
-    const int64_t nb = std::min(chunk, B - b0);
-    PK_CUDA(cudaMemcpyAsync(S.st_q + b0 * m->nq, q_host + b0 * m->nq, sizeof(float) * nb * m->nq,
-                            cudaMemcpyHostToDevice, s_in));
-    if (ts > 0)
-      PK_CUDA(cudaMemcpyAsync(S.st_t + b0 * ts, targets_host + b0 * ts, sizeof(float) * nb * ts,
-                              cudaMemcpyHostToDevice, s_in));
+    if (upload(k, s_in)) return 1;
     PK_CUDA(cudaEventRecord(S.st_in[k], s_in));
     PK_CUDA(cudaStreamWaitEvent(s_k, S.st_in[k], 0));
-    if (solve_device(m, pr, S.st_q + b0 * m->nq, S.st_t + b0 * ts, S.st_v + b0 * m->nv, S.st_s + b0, nb, s_k))
-      return 1;
-    PK_CUDA(cudaEventRecord(S.st_kern[k], s_k));
+    if (solve(k, direct ? v_dev : S.st_v, direct ? s_dev : S.st_s, s_k)) return 1;
+    if (!direct) PK_CUDA(cudaEventRecord(S.st_kern[k], s_k));
   }
-  // downloads start once the last upload is through (st_in[nchunks-1] on the in-order s_in)
-  PK_CUDA(cudaStreamWaitEvent(s_out, S.st_in[nchunks - 1], 0));
-  for (int64_t k = 0; k < nchunks; ++k) {
-    const int64_t b0 = k * chunk;
-    const int64_t nb = std::min(chunk, B - b0);
-    PK_CUDA(cudaStreamWaitEvent(s_out, S.st_kern[k], 0));
-    PK_CUDA(cudaMemcpyAsync(v_host + b0 * m->nv, S.st_v + b0 * m->nv, sizeof(float) * nb * m->nv,
-                            cudaMemcpyDeviceToHost, s_out));
-    if (status_host)
-      PK_CUDA(cudaMemcpyAsync(status_host + b0, S.st_s + b0, sizeof(int32_t) * nb, cudaMemcpyDeviceToHost, s_out));
+  if (!direct) {
+    // downloads start once the last upload is through (st_in[nchunks-1] on the in-order s_in)
+    PK_CUDA(cudaStreamWaitEvent(s_out, S.st_in[nchunks - 1], 0));
+    for (int64_t k = 0; k < nchunks; ++k) {
+      PK_CUDA(cudaStreamWaitEvent(s_out, S.st_kern[k], 0));
+      if (download(k, s_out)) return 1;
+    }
   }
   // the caller's stream resumes when everything is back; s_in / s_k are ordered before s_out
-  PK_CUDA(cudaEventRecord(S.st_join[2], s_out));
+  PK_CUDA(cudaEventRecord(S.st_join[2], direct ? s_k : s_out));
   PK_CUDA(cudaStreamWaitEvent(stream, S.st_join[2], 0));
   return 0;
 }
@@ -1356,7 +1198,7 @@ extern "C" int pk_build_ik_batched(const PkModel* m, const PkProblemDesc* prob, 
   A.c = c;
   A.h = h;
   A.task_index = -1;
-  return launch_generic(m, P, A, B, (cudaStream_t)stream);
+  return launch_generic(m, pr.sel.generic_class, P, A, B, (cudaStream_t)stream);
 }
 
 extern "C" int pk_constraint_rows_batched(const PkModel* m, const PkProblemDesc* prob, const float* q,
@@ -1379,7 +1221,7 @@ extern "C" int pk_constraint_rows_batched(const PkModel* m, const PkProblemDesc*
   A.lo = lo;
   A.hi = hi;
   A.task_index = -1;
-  return launch_generic(m, pr.P, A, B, (cudaStream_t)stream);
+  return launch_generic(m, pr.sel.generic_class, pr.P, A, B, (cudaStream_t)stream);
 }
 
 extern "C" int pk_task_terms_batched(const PkModel* m, const PkProblemDesc* prob, int32_t task_index,
@@ -1397,28 +1239,22 @@ extern "C" int pk_task_terms_batched(const PkModel* m, const PkProblemDesc* prob
   A.e = e;
   A.J = J;
   A.task_index = task_index;
-  const int type = P.tasks[task_index].type;
-  A.task_k = type == PK_TASK_COM ? 3
-             : type == PK_TASK_LINEAR ? P.tasks[task_index].rows
-                                      : (pk::is_diag_task(type) ? m->nv - (m->free_flyer ? 6 : 0) : 6);
+  A.task_k = pk::task_terms_rows(m->hm, P.tasks[task_index]);
   // H must be accumulated for the task loop to run; give the kernel no v/H outputs
   // but keep ntasks > 0 so the loop executes
-  return launch_generic(m, P, A, B, (cudaStream_t)stream);
+  return launch_generic(m, pr.sel.generic_class, P, A, B, (cudaStream_t)stream);
 }
 
 extern "C" int pk_forward_kinematics_batched(const PkModel* m, const float* q, float* oMf, float* com,
                                              int64_t B, void* stream) {
   if (check_common(m, q, B)) return 1;
   if (B == 0) return 0;
-  pk::DevProblem P;
-  memset(&P, 0, sizeof(P));
-  for (int i = 0; i < PK_MAX_NV; ++i) { P.chk_lo[i] = -INFINITY; P.chk_hi[i] = INFINITY; }
   pk::GenericArgs A{};
   A.q = q;
   A.oMf = oMf;
   A.com = com;
   A.task_index = -1;
-  return launch_generic(m, P, A, B, (cudaStream_t)stream);
+  return launch_generic(m, pk::generic_size_class(m->hm), pk::kinematics_problem(), A, B, (cudaStream_t)stream);
 }
 
 extern "C" int pk_frame_jacobian_batched(const PkModel* m, int32_t frame, const float* q, float* J, int64_t B,
@@ -1426,15 +1262,12 @@ extern "C" int pk_frame_jacobian_batched(const PkModel* m, int32_t frame, const 
   if (check_common(m, q, B)) return 1;
   if (frame < 0 || frame >= m->nframes) return fail("frame index out of range");
   if (B == 0) return 0;
-  pk::DevProblem P;
-  memset(&P, 0, sizeof(P));
-  for (int i = 0; i < PK_MAX_NV; ++i) { P.chk_lo[i] = -INFINITY; P.chk_hi[i] = INFINITY; }
   pk::GenericArgs A{};
   A.q = q;
   A.Jf = J;
   A.jac_frame = frame;
   A.task_index = -1;
-  return launch_generic(m, P, A, B, (cudaStream_t)stream);
+  return launch_generic(m, pk::generic_size_class(m->hm), pk::kinematics_problem(), A, B, (cudaStream_t)stream);
 }
 
 extern "C" int pk_integrate_batched(const PkModel* m, const float* q, const float* v, float dt, float* q_out,
@@ -1446,7 +1279,5 @@ extern "C" int pk_integrate_batched(const PkModel* m, const float* q, const floa
   const int64_t grid = (B + block - 1) / block;
   pk::integrate_kernel<<<(unsigned)grid, block, 0, (cudaStream_t)stream>>>(m->nq, m->nv, m->free_flyer, q, v, dt,
                                                                              q_out, B);
-  g_launches.fetch_add(1);
-  PK_CUDA(cudaGetLastError());
-  return 0;
+  return launched();
 }

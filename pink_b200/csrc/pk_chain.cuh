@@ -23,6 +23,8 @@
 namespace pk {
 
 constexpr int kChainMaxFrameTasks = 2;
+// longest targets row the PDL instantiation of ik_chain_kernel copies: frame targets, posture and dq_prev
+PK_HD constexpr int chain_row_words(int nj, int nft) { return 12 * nft + 2 * nj; }
 
 struct ChainJoint {
   float X[12];  // placement in the parent joint frame, row-major [R | p]

@@ -105,6 +105,57 @@ struct GenericOut {
   float* hi;       // [nv]
 };
 
+// The same outputs for a whole batch (rows of instance i at i times the row sizes above), with
+// the inputs; task_k = rows of task `task_index`.
+struct GenericArgs {
+  const float* q;
+  const float* targets;
+  float* v;
+  int32_t* status;
+  float* H;
+  float* c;
+  float* h;
+  float* e;
+  float* J;
+  int task_index;
+  int task_k;
+  float* oMf;
+  float* com;
+  float* Jf;
+  int jac_frame;
+  float* G;
+  float* hG;
+  float* E;
+  float* f;
+  float* lo;
+  float* hi;
+};
+
+// Outputs of instance i.
+PK_HD GenericOut generic_out(const DevModel& M, const GenericArgs& A, int64_t i) {
+  const int nv = M.nv;
+  GenericOut out;
+  out.v = A.v ? A.v + i * nv : nullptr;
+  out.status = A.status ? A.status + i : nullptr;
+  out.H = A.H ? A.H + i * nv * nv : nullptr;
+  out.c = A.c ? A.c + i * nv : nullptr;
+  out.h = A.h ? A.h + i * 4 * nv : nullptr;
+  out.e = A.e ? A.e + i * A.task_k : nullptr;
+  out.J = A.J ? A.J + i * A.task_k * nv : nullptr;
+  out.task_index = A.task_index;
+  out.oMf = A.oMf ? A.oMf + i * M.nframes * 12 : nullptr;
+  out.com = A.com ? A.com + i * 3 : nullptr;
+  out.Jf = A.Jf ? A.Jf + i * 6 * nv : nullptr;
+  out.jac_frame = A.jac_frame;
+  out.G = A.G ? A.G + i * PK_MAX_INEQ_ROWS * nv : nullptr;
+  out.hG = A.hG ? A.hG + i * PK_MAX_INEQ_ROWS : nullptr;
+  out.E = A.E ? A.E + i * PK_MAX_EQ_ROWS * nv : nullptr;
+  out.f = A.f ? A.f + i * PK_MAX_EQ_ROWS : nullptr;
+  out.lo = A.lo ? A.lo + i * nv : nullptr;
+  out.hi = A.hi ? A.hi + i * nv : nullptr;
+  return out;
+}
+
 // stacked task rows: 6 per frame task, 3 per CoM task; every task set the ABI can describe fits
 // (nothing is ever truncated)
 constexpr int kGenericMaxRows = 6 * PK_MAX_TASKS;

@@ -173,6 +173,22 @@ inline int task_row_count(const HostModel& m, const DevTask& d) {
   return 6;
 }
 
+// Rows of e and J that the task-terms export writes for task `d`.
+inline int task_terms_rows(const HostModel& m, const DevTask& d) {
+  return is_diag_task(d.type) ? m.nv - (m.free_flyer ? 6 : 0) : task_row_count(m, d);
+}
+
+// Problem of the forward-kinematics and frame-Jacobian exports: no tasks, no limits.
+inline DevProblem kinematics_problem() {
+  DevProblem P;
+  memset(&P, 0, sizeof(P));
+  for (int i = 0; i < PK_MAX_NV; ++i) {
+    P.chk_lo[i] = -INFINITY;
+    P.chk_hi[i] = INFINITY;
+  }
+  return P;
+}
+
 inline std::string make_dev_problem(const HostModel& m, const PkProblemDesc* p, DevProblem* out,
                                     HostExtras* hx = nullptr) {
   if (!p) return "null problem";

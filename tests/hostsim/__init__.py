@@ -9,6 +9,7 @@ the fp64 oracle without a GPU.
 import ctypes as C
 import os
 import subprocess
+from collections import namedtuple
 
 import numpy as np
 
@@ -53,6 +54,13 @@ def _p(a):
     return None if a is None else a.ctypes.data_as(C.c_void_p)
 
 
+# The CUDA library's kernel selection for a problem (pk_select.hpp): path "chain" / "tree" /
+# "general"; the chain kernels' <NJ, NFT>; generic = <NJMAX, NVMAX> of ik_generic_kernel; lanes per
+# instance of the sub-warp chain kernel (0: ik_chain_kernel); pdl_row_fits: the targets row fits the
+# PDL chain kernel's copy; K: task rows of the tree plan.
+Selection = namedtuple("Selection", "path nj nft generic lanes pdl_row_fits K")
+
+
 class HostSim:
     """Runs the kernel bodies on the CPU for one model."""
 
@@ -85,17 +93,26 @@ class HostSim:
         return a
 
     def solve_ik(self, prob, q, targets=None, general_path=False, path=None):
+        """path: see hs_solve_ik; ``self.selection`` is the kernel selection the body ran."""
         q = self._f32(q)
         B = q.shape[0]
         t = None if targets is None else self._f32(targets)
         v = np.zeros((B, self.nv), dtype=np.float32)
         st = np.zeros(B, dtype=np.int32)
-        used = C.c_int(0)
+        sel = (C.c_int * 8)()
         self._chk(lib().hs_solve_ik(self.handle, C.byref(prob), _p(q), _p(t), _p(v), _p(st),
-                                    C.c_int64(B), (1 if general_path else 0) if path is None else path, C.byref(used)))
-        self.used_chain = used.value == 1
-        self.used_tree = used.value == 2
+                                    C.c_int64(B), (1 if general_path else 0) if path is None else path, sel))
+        self.selection = Selection(("chain", "tree", "general")[sel[0]], sel[1], sel[2], (sel[3], sel[4]), sel[5],
+                                   bool(sel[6]), sel[7])
         return v, st
+
+    @property
+    def used_chain(self):
+        return self.selection.path == "chain"
+
+    @property
+    def used_tree(self):
+        return self.selection.path == "tree"
 
     def build_ik(self, prob, q, targets=None):
         q = self._f32(q)

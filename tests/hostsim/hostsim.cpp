@@ -9,92 +9,55 @@
 #include <vector>
 
 #include "../../include/pink_b200.h"
-#include "../../pink_b200/csrc/pk_marshal.hpp"
+#include "../../pink_b200/csrc/pk_select.hpp"
 #include "../../pink_b200/csrc/pk_dualqp.cuh"
 
 namespace {
 thread_local std::string g_err;
 int fail(const std::string& m) { g_err = m; return 1; }
 
-template <int NJ>
-void run_chain(const pk::HostModel& hm, const pk::DevProblem& P, const float* q, const float* targets, float* v,
-               int32_t* status, int64_t B) {
-  pk::ChainParams<NJ> C;
-  pk::make_chain_params<NJ>(hm, P, &C, P.ext);
-  for (int64_t i = 0; i < B; ++i) {
-    float qi[NJ], vi[NJ];
-    for (int k = 0; k < NJ; ++k) qi[k] = q[i * NJ + k];
-    int st = 0;
-    const float* trow = targets + i * (int64_t)P.target_stride;
-    switch (C.n_frame_tasks) {
-      case 0: pk::ik_step_chain<NJ, 0>(C, qi, trow, vi, st); break;
-      case 1: pk::ik_step_chain<NJ, 1>(C, qi, trow, vi, st); break;
-      default: pk::ik_step_chain<NJ, 2>(C, qi, trow, vi, st); break;
+// The bodies of the kernels a chain selection names, lanes emulated by loops in the sub-warp one.
+template <int NJ, int NFT>
+void run_chain(const pk::HostModel& hm, const pk::DevProblem& P, const pk::Selection& sel, const float* q,
+               const float* targets, float* v, int32_t* status, int64_t B) {
+  if (!sel.lanes) {
+    pk::ChainParams<NJ> C;
+    pk::make_chain_params<NJ>(hm, P, &C, P.ext);
+    for (int64_t i = 0; i < B; ++i) {
+      float qi[NJ], vi[NJ];
+      for (int k = 0; k < NJ; ++k) qi[k] = q[i * NJ + k];
+      int st = 0;
+      pk::ik_step_chain<NJ, NFT>(C, qi, targets + i * (int64_t)P.target_stride, vi, st);
+      for (int k = 0; k < NJ; ++k) v[i * NJ + k] = vi[k];
+      if (status) status[i] = st;
     }
-    for (int k = 0; k < NJ; ++k) v[i * NJ + k] = vi[k];
-    if (status) status[i] = st;
+    return;
   }
+  pk::with_lanes<NJ, NFT>(sel.lanes, [&](auto lanes) {
+    constexpr int L = decltype(lanes)::value;
+    using Step = pk::CoopStep<NJ, NFT, L>;
+    typename Step::Params C;
+    pk::make_coop_params<NJ, L>(hm, P, &C, P.ext);
+    const pk::Group<L> G{};
+    auto jc = [&](int j) -> const pk::CoopJoint& { return C.joint[j]; };
+    for (int64_t i = 0; i < B; ++i) {
+      pk::GVar<typename Step::Lane, L> S;
+      for (int h = 0; h < L; ++h)
+        for (int k = 0; k < Step::NC; ++k) {
+          const int j = h * Step::NC + k;
+          S[h].q[k] = j < NJ ? q[i * NJ + j] : 0.f;
+        }
+      int st = 0;
+      pk::ik_step_coop<NJ, NFT, L>(G, C, jc, targets + i * (int64_t)P.target_stride, S, st);
+      for (int h = 0; h < L; ++h)
+        for (int k = 0; k < Step::NC; ++k) {
+          const int j = h * Step::NC + k;
+          if (j < NJ) v[i * NJ + j] = S[h].x[k];
+        }
+      if (status) status[i] = st;
+    }
+  });
 }
-
-// Sub-warp chain kernel body (pk_coop.cuh) with L lanes per instance, lanes emulated by loops.
-template <int NJ, int NFT, int L>
-void run_coop_nft(const pk::HostModel& hm, const pk::DevProblem& P, const float* q, const float* targets, float* v,
-                  int32_t* status, int64_t B) {
-  using Step = pk::CoopStep<NJ, NFT, L>;
-  typename Step::Params C;
-  pk::make_coop_params<NJ, L>(hm, P, &C, P.ext);
-  const pk::Group<L> G{};
-  auto jc = [&](int j) -> const pk::CoopJoint& { return C.joint[j]; };
-  for (int64_t i = 0; i < B; ++i) {
-    pk::GVar<typename Step::Lane, L> S;
-    for (int h = 0; h < L; ++h)
-      for (int k = 0; k < Step::NC; ++k) {
-        const int j = h * Step::NC + k;
-        S[h].q[k] = j < NJ ? q[i * NJ + j] : 0.f;
-      }
-    int st = 0;
-    const float* trow = targets + i * (int64_t)P.target_stride;
-    pk::ik_step_coop<NJ, NFT, L>(G, C, jc, trow, S, st);
-    for (int h = 0; h < L; ++h)
-      for (int k = 0; k < Step::NC; ++k) {
-        const int j = h * Step::NC + k;
-        if (j < NJ) v[i * NJ + j] = S[h].x[k];
-      }
-    if (status) status[i] = st;
-  }
-}
-
-template <int NJ, int L>
-void run_coop(const pk::HostModel& hm, const pk::DevProblem& P, const float* q, const float* targets, float* v,
-              int32_t* status, int64_t B) {
-  int nft = 0;
-  for (int t = 0; t < P.ntasks; ++t) nft += P.tasks[t].type == PK_TASK_FRAME;
-  switch (nft) {
-    case 0: run_coop_nft<NJ, 0, L>(hm, P, q, targets, v, status, B); break;
-    case 1: run_coop_nft<NJ, 1, L>(hm, P, q, targets, v, status, B); break;
-    default: run_coop_nft<NJ, 2, L>(hm, P, q, targets, v, status, B); break;
-  }
-}
-
-template <int L>
-bool run_coop_nj(const pk::HostModel& hm, const pk::DevProblem& P, const float* q, const float* targets, float* v,
-                 int32_t* status, int64_t B) {
-  switch (hm.njoints) {
-    case 2: run_coop<2, L>(hm, P, q, targets, v, status, B); return true;
-    case 3: run_coop<3, L>(hm, P, q, targets, v, status, B); return true;
-    case 4: run_coop<4, L>(hm, P, q, targets, v, status, B); return true;
-    case 5: run_coop<5, L>(hm, P, q, targets, v, status, B); return true;
-    case 6: run_coop<6, L>(hm, P, q, targets, v, status, B); return true;
-    case 7: run_coop<7, L>(hm, P, q, targets, v, status, B); return true;
-  }
-  return false;
-}
-
-struct Args {
-  const float* q; const float* targets; float* v; int32_t* status; float* H; float* c; float* h;
-  float* e; float* J; int task_index; int task_k; float* oMf; float* com; float* Jf; int jac_frame;
-  float* G; float* hG; float* E; float* f; float* lo; float* hi;
-};
 
 // make_dev_problem + host image of the optional parts, wired through P.ext
 std::string make_problem(const pk::HostModel& hm, const PkProblemDesc* prob, pk::DevProblem* P, pk::HostExtras* hx) {
@@ -103,32 +66,15 @@ std::string make_problem(const pk::HostModel& hm, const PkProblemDesc* prob, pk:
   return e;
 }
 
-void run_generic(const pk::HostModel& hm, const pk::DevProblem& P, const Args& A, int64_t B) {
+// ik_generic_kernel's body at the instantiation the CUDA library launches for this model
+void run_generic(const pk::HostModel& hm, const pk::DevProblem& P, const pk::GenericArgs& A, int64_t B) {
   const pk::DevModel M = hm.host_view();
-  const int nv = M.nv;
-  static thread_local pk::Generic<PK_MAX_JOINTS, PK_MAX_NV> G;
-  for (int64_t i = 0; i < B; ++i) {
-    pk::GenericOut out;
-    out.v = A.v ? A.v + i * nv : nullptr;
-    out.status = A.status ? A.status + i : nullptr;
-    out.H = A.H ? A.H + i * nv * nv : nullptr;
-    out.c = A.c ? A.c + i * nv : nullptr;
-    out.h = A.h ? A.h + i * 4 * nv : nullptr;
-    out.e = A.e ? A.e + i * A.task_k : nullptr;
-    out.J = A.J ? A.J + i * A.task_k * nv : nullptr;
-    out.task_index = A.task_index;
-    out.oMf = A.oMf ? A.oMf + i * M.nframes * 12 : nullptr;
-    out.com = A.com ? A.com + i * 3 : nullptr;
-    out.Jf = A.Jf ? A.Jf + i * 6 * nv : nullptr;
-    out.jac_frame = A.jac_frame;
-    out.G = A.G ? A.G + i * PK_MAX_INEQ_ROWS * nv : nullptr;
-    out.hG = A.hG ? A.hG + i * PK_MAX_INEQ_ROWS : nullptr;
-    out.E = A.E ? A.E + i * PK_MAX_EQ_ROWS * nv : nullptr;
-    out.f = A.f ? A.f + i * PK_MAX_EQ_ROWS : nullptr;
-    out.lo = A.lo ? A.lo + i * nv : nullptr;
-    out.hi = A.hi ? A.hi + i * nv : nullptr;
-    G.step(M, P, A.q + i * M.nq, A.targets ? A.targets + i * (int64_t)P.target_stride : nullptr, out);
-  }
+  pk::with_generic(pk::generic_size_class(hm), [&](auto nj, auto nv) {
+    static thread_local pk::Generic<decltype(nj)::value, decltype(nv)::value> G;
+    for (int64_t i = 0; i < B; ++i)
+      G.step(M, P, A.q + i * M.nq, A.targets ? A.targets + i * (int64_t)P.target_stride : nullptr,
+             pk::generic_out(M, A, i));
+  });
 }
 }  // namespace
 
@@ -145,58 +91,48 @@ int hs_model_create(const PkModelDesc* d, void** out) {
 }
 void hs_model_destroy(void* m) { delete (pk::HostModel*)m; }
 
-// path: 0 auto (same selection as the CUDA library), 1 force the general path, 2 force the tree kernel body
+// The kernel body the CUDA library's selection (pk_select.hpp) names for this problem.
+// path: 0 the library's default options, 1 PK_FORCE_GENERIC=1, 2 without the chain kernels (the
+// tree kernel body on a chain), 11 / 12 / 14 / 18 PK_CHAIN_LANES = 1 / 2 / 4 / 8 (the problem must
+// take a chain kernel).  sel_out: path (pk::KernelPath), nj, nft, the general path's <NJMAX, NVMAX>,
+// lanes, PDL row fits, tree task rows K.
 int hs_solve_ik(void* model, const PkProblemDesc* prob, const float* q, const float* targets, float* v,
-                int32_t* status, int64_t B, int path, int* used_chain) {
+                int32_t* status, int64_t B, int path, int* sel_out) {
   const pk::HostModel& hm = *(pk::HostModel*)model;
   pk::DevProblem P;
   pk::HostExtras hx;
   const std::string e = make_problem(hm, prob, &P, &hx);
   if (!e.empty()) return fail(e);
-  const bool chain = path == 0 && pk::chain_eligible(hm, P, hx.present && !hx.box_only());
-  if (used_chain) *used_chain = chain ? 1 : 0;
-  // path 11 / 12 / 14 / 18: the sub-warp chain kernel body with 1 / 2 / 4 / 8 lanes per instance
-  if (path > 10) {
-    if (!pk::chain_eligible(hm, P, hx.present && !hx.box_only())) return fail("problem does not fit the chain kernel");
-    if (used_chain) *used_chain = 1;
-    bool ok = false;
-    switch (path - 10) {
-      case 1: ok = run_coop_nj<1>(hm, P, q, targets, v, status, B); break;
-      case 2: ok = run_coop_nj<2>(hm, P, q, targets, v, status, B); break;
-      case 4: ok = run_coop_nj<4>(hm, P, q, targets, v, status, B); break;
-      case 8: ok = run_coop_nj<8>(hm, P, q, targets, v, status, B); break;
-    }
-    return ok ? 0 : fail("unsupported lanes per instance");
+  pk::SelectOptions o;
+  o.use_chain = path == 0 || path > 10;
+  o.use_tree = path != 1;
+  o.chain_lanes = path > 10 ? path - 10 : 0;
+  const pk::Selection sel = pk::select_kernel(hm, P, hx, o);
+  const int report[] = {sel.path, sel.nj, sel.nft, 0, 0, sel.lanes, sel.pdl_row_fits, sel.plan.K};
+  std::memcpy(sel_out, report, sizeof(report));
+  pk::with_generic(sel.generic_class, [&](auto nj, auto nv) { sel_out[3] = nj; sel_out[4] = nv; });
+  if (path > 10 && sel.path != pk::kPathChain) return fail("problem does not fit the chain kernel");
+  if (path == 2 && sel.path != pk::kPathTree) return fail("problem does not fit the tree kernel");
+  if (sel.path == pk::kPathChain) {
+    pk::with_nj(sel.nj, [&](auto nj) {
+      pk::with_nft(sel.nft, [&](auto nft) {
+        run_chain<decltype(nj)::value, decltype(nft)::value>(hm, P, sel, q, targets, v, status, B);
+      });
+    });
+  } else if (sel.path == pk::kPathTree) {
+    const pk::TreePlan& L = sel.plan;
+    const pk::DevModel M = hm.host_view();
+    std::vector<float> W(L.words + 8);
+    float* Wp = W.data();
+    if (((uintptr_t)Wp & 7) != 0) ++Wp;  // the dual method keeps doubles in the workspace
+    for (int64_t i = 0; i < B; ++i)
+      pk::TreeStep::run(M, P, L, q + i * L.nq, targets ? targets + i * (int64_t)L.stride : nullptr, Wp,
+                        v + i * L.nv, status ? status + i : nullptr);
+  } else {
+    pk::GenericArgs A{};
+    A.q = q; A.targets = targets; A.v = v; A.status = status; A.task_index = -1;
+    run_generic(hm, P, A, B);
   }
-  if (chain) {
-    switch (hm.njoints) {
-      case 2: run_chain<2>(hm, P, q, targets, v, status, B); return 0;
-      case 3: run_chain<3>(hm, P, q, targets, v, status, B); return 0;
-      case 4: run_chain<4>(hm, P, q, targets, v, status, B); return 0;
-      case 5: run_chain<5>(hm, P, q, targets, v, status, B); return 0;
-      case 6: run_chain<6>(hm, P, q, targets, v, status, B); return 0;
-      case 7: run_chain<7>(hm, P, q, targets, v, status, B); return 0;
-    }
-  }
-  if (path == 2 || (path == 0 && !chain)) {
-    bool ok = false;
-    const pk::TreePlan L = pk::make_tree_plan(hm, P, &ok, hx.present ? &hx.X : nullptr);
-    if (ok) {
-      if (used_chain) *used_chain = 2;
-      const pk::DevModel M = hm.host_view();
-      std::vector<float> W(L.words + 8);
-      float* Wp = W.data();
-      if (((uintptr_t)Wp & 7) != 0) ++Wp;  // the dual method keeps doubles in the workspace
-      for (int64_t i = 0; i < B; ++i)
-        pk::TreeStep::run(M, P, L, q + i * L.nq, targets ? targets + i * (int64_t)L.stride : nullptr, Wp,
-                          v + i * L.nv, status ? status + i : nullptr);
-      return 0;
-    }
-    if (path == 2) return fail("problem does not fit the tree kernel");
-  }
-  Args A{};
-  A.q = q; A.targets = targets; A.v = v; A.status = status; A.task_index = -1;
-  run_generic(hm, P, A, B);
   return 0;
 }
 
@@ -207,7 +143,7 @@ int hs_build_ik(void* model, const PkProblemDesc* prob, const float* q, const fl
   pk::HostExtras hx;
   const std::string e = make_problem(hm, prob, &P, &hx);
   if (!e.empty()) return fail(e);
-  Args A{};
+  pk::GenericArgs A{};
   A.q = q; A.targets = targets; A.H = H; A.c = c; A.h = h; A.task_index = -1;
   run_generic(hm, P, A, B);
   return 0;
@@ -220,7 +156,7 @@ int hs_constraint_rows(void* model, const PkProblemDesc* prob, const float* q, c
   pk::HostExtras hx;
   const std::string e = make_problem(hm, prob, &P, &hx);
   if (!e.empty()) return fail(e);
-  Args A{};
+  pk::GenericArgs A{};
   A.q = q; A.targets = targets; A.G = G; A.hG = hG; A.E = E; A.f = f; A.lo = lo; A.hi = hi; A.task_index = -1;
   run_generic(hm, P, A, B);
   return 0;
@@ -234,36 +170,27 @@ int hs_task_terms(void* model, const PkProblemDesc* prob, int task_index, const 
   const std::string e = make_problem(hm, prob, &P, &hx);
   if (!e.empty()) return fail(e);
   if (task_index < 0 || task_index >= P.ntasks) return fail("task_index out of range");
-  Args A{};
+  pk::GenericArgs A{};
   A.q = q; A.targets = targets; A.e = eo; A.J = J; A.task_index = task_index;
-  const int type = P.tasks[task_index].type;
-  A.task_k = type == PK_TASK_COM ? 3
-             : type == PK_TASK_LINEAR ? P.tasks[task_index].rows
-                                      : (pk::is_diag_task(type) ? hm.nv - (hm.free_flyer ? 6 : 0) : 6);
+  A.task_k = pk::task_terms_rows(hm, P.tasks[task_index]);
   run_generic(hm, P, A, B);
   return 0;
 }
 
 int hs_forward_kinematics(void* model, const float* q, float* oMf, float* com, int64_t B) {
   const pk::HostModel& hm = *(pk::HostModel*)model;
-  pk::DevProblem P;
-  memset(&P, 0, sizeof(P));
-  for (int i = 0; i < PK_MAX_NV; ++i) { P.chk_lo[i] = -INFINITY; P.chk_hi[i] = INFINITY; }
-  Args A{};
+  pk::GenericArgs A{};
   A.q = q; A.oMf = oMf; A.com = com; A.task_index = -1;
-  run_generic(hm, P, A, B);
+  run_generic(hm, pk::kinematics_problem(), A, B);
   return 0;
 }
 
 int hs_frame_jacobian(void* model, int frame, const float* q, float* J, int64_t B) {
   const pk::HostModel& hm = *(pk::HostModel*)model;
   if (frame < 0 || frame >= hm.nframes) return fail("frame index out of range");
-  pk::DevProblem P;
-  memset(&P, 0, sizeof(P));
-  for (int i = 0; i < PK_MAX_NV; ++i) { P.chk_lo[i] = -INFINITY; P.chk_hi[i] = INFINITY; }
-  Args A{};
+  pk::GenericArgs A{};
   A.q = q; A.Jf = J; A.jac_frame = frame; A.task_index = -1;
-  run_generic(hm, P, A, B);
+  run_generic(hm, pk::kinematics_problem(), A, B);
   return 0;
 }
 

@@ -170,12 +170,11 @@ def host_side(case):
     hs = HostSim(sc.model)
     prob, targets, _ = sc.problem()
     v_h, st_h = hs.solve_ik(prob, sc.q32, targets)
-    landed = "chain" if hs.used_chain else "tree" if hs.used_tree else "general"
-    assert landed == case.kernel, (landed, case.kernel)
-    nv, nj = sc.table.nv, sc.table.njoints
-    if case.inst is not None:  # launch_generic's choice
-        inst = "<8, 8>" if nv <= 8 and nj <= 8 else "<30, 36>" if nv <= 36 and nj <= 30 else "<58, 64>"
-        assert inst == case.inst, (inst, nv, nj)
+    assert hs.selection.path == case.kernel, (hs.selection, case.kernel)
+    nv = sc.table.nv
+    if case.inst is not None:
+        inst = "<%d, %d>" % hs.selection.generic
+        assert inst == case.inst, (inst, nv, sc.table.njoints)
     if case.qp is not None:
         dual = prob.nbarriers > 0 or prob.nconstraints > 0 or prob.fb_enabled
         assert ("dual" if dual else "box") == case.qp
@@ -298,16 +297,6 @@ CHAINS = {
 ROLLOUT_STEPS = 4
 
 
-def _nft(sc):
-    return sum(type(t).__name__ == "FrameTask" for t in sc.tasks)
-
-
-def coop_takes(lanes, sc):
-    """Does the library run ik_coop_kernel for PK_CHAIN_LANES = lanes?  4 and 8 lanes exist for
-    <6, 1> only; other shapes fall back to the thread-per-instance kernel."""
-    return lanes in (1, 2) or (sc.table.njoints == 6 and _nft(sc) == 1)
-
-
 def dump_chain_outputs(path, steps=ROLLOUT_STEPS):
     """Solve and rollout(steps, q_out) of every CHAINS case on cuda:0 (run in a subprocess:
     PK_CHAIN_LANES / PK_CHAIN_FORCE_RECOMPUTE are read once per process)."""
@@ -358,8 +347,8 @@ def host_rollout(hs, prob, sc, targets, path, steps=ROLLOUT_STEPS):
 
 
 def chain_host_side(name, lanes):
-    """Dispatch (chain kernel; the host build runs the L-lane body) and the host build of the
-    sub-warp kernel against the oracle."""
+    """Dispatch (chain kernel; the host build runs the body PK_CHAIN_LANES = L selects: the L-lane
+    one, or for L = 4 / 8 off <6, 1> the thread-per-instance one) against the oracle."""
     from tests.hostsim import HostSim
 
     sc = CHAINS[name]()
@@ -392,7 +381,7 @@ def test_sub_warp_chain_kernel(lanes, tmp_path, default_chain_outputs):
     for name in CHAINS:
         sc, hs, prob, targets, v_h, st_h, v_ref, st_ref = chain_host_side(name, lanes)
         g = {k: got[f"{name}/{k}"] for k in ("v", "status", "q_out", "v_roll", "status_roll")}
-        if not coop_takes(lanes, sc):
+        if hs.selection.lanes != lanes:  # no L-lane variant for this shape
             for k, val in g.items():
                 np.testing.assert_array_equal(val, default_chain_outputs[f"{name}/{k}"], err_msg=f"{name} {k}")
             continue
@@ -454,9 +443,8 @@ def recompute_dispatch(name):
     prob, targets, _ = sc.problem()
     hs.solve_ik(prob, sc.q32[:1], None if targets is None else targets[:1])
     assert hs.used_chain
-    nj, nft = sc.table.njoints, _nft(sc)
-    assert name.startswith(f"nj{nj}-nft{nft}")
-    assert prob.target_stride <= 12 * nft + 2 * nj
+    assert name.startswith(f"nj{hs.selection.nj}-nft{hs.selection.nft}")
+    assert hs.selection.pdl_row_fits
     return prob
 
 

@@ -2,7 +2,9 @@
 lanes-per-instance variant L = 1, 2, 4, 8 (hostsim path 10 + L), against the fp64 oracle:
 the same scenarios as the one-instance-per-thread kernel in test_hostsim_parity.py, plus
 the KKT certificate at a large batch and the interior regime (loose limits, where the
-solver leaves the two-slot loop for the Cholesky rounds)."""
+solver leaves the two-slot loop for the Cholesky rounds).  The host build follows the library's
+selection: L = 4 / 8 exist at <6, 1> only, so on other chains those cases run the
+thread-per-instance kernel the library falls back to."""
 
 import numpy as np
 import pytest
