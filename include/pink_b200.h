@@ -237,6 +237,29 @@ int pk_rollout_prepared(const PkModel* model, const PkProblem* problem,
                         float* q_out, float* v, int32_t* status, int64_t B,
                         void* stream);
 
+/* Trajectory rollout: n_steps iterations of  v = solve_ik(q, targets_s); q <- q (+) v dt,
+ * where the targets row of instance i at step s is
+ *   targets + s * target_step + i * target_stride
+ * (target_step in floats, >= 0; 0 = the same row every step, as pk_rollout_prepared).
+ * q_out[B][nq] final q (may alias q), v[B][nv] velocity of the last step that ran,
+ * status[B] = OR over the steps that ran (may be NULL).
+ * Optional records (NULL = not written), step-major:
+ *   q_traj[n_steps][B][nq]  q after step s,
+ *   v_traj[n_steps][B][nv]  velocity of step s,
+ *   status_traj[n_steps][B] OR of the statuses of steps 0..s.
+ * Every path freezes an instance that fails a step (NO_SOLUTION / NOT_POSDEF, or
+ * OUT_OF_LIMITS with safety_break): from then on q stays, v_traj rows are 0 and
+ * status_traj repeats.  One launch on every path (chains, joint trees and the general
+ * path); no host synchronisation and no allocation, so the call can be captured in a
+ * CUDA graph.  The dq_prev words of AccelerationLimit / LowAccelerationTask are read
+ * from each step's targets row as given: the rollout does not feed its own previous
+ * velocity back into them.                                                            */
+int pk_rollout_trajectory_prepared(const PkModel* model, const PkProblem* problem,
+                                   const float* q, const float* targets, int64_t target_step,
+                                   int32_t n_steps, float* q_out, float* v, int32_t* status,
+                                   float* q_traj, float* v_traj, int32_t* status_traj,
+                                   int64_t B, void* stream);
+
 /* ---- multi-GPU: all-gather of v through NVLink peer memory (SURVEY.md section 8e) ----
  * One process per GPU; instances are independent, so the only exchange is the one
  * BASELINE north_star names: collecting v.  Instead of a collective after the kernel, the

@@ -192,6 +192,8 @@ def declare(lib: C.CDLL, prefix: str = "pk_") -> None:
     lib.pk_solve_ik_prepared.argtypes = [C.c_void_p, C.c_void_p, _FP, _FP, _FP, _FP, C.c_int64, C.c_void_p]
     lib.pk_solve_ik_prepared_host.argtypes = [C.c_void_p, C.c_void_p, _FP, _FP, _FP, _FP, C.c_int64, C.c_void_p]
     lib.pk_rollout_prepared.argtypes = [C.c_void_p, C.c_void_p, _FP, _FP, C.c_int32, _FP, _FP, _FP, C.c_int64, C.c_void_p]
+    lib.pk_rollout_trajectory_prepared.argtypes = [C.c_void_p, C.c_void_p, _FP, _FP, C.c_int64, C.c_int32, _FP, _FP, _FP,
+                                                   _FP, _FP, _FP, C.c_int64, C.c_void_p]
     lib.pk_build_ik_batched.argtypes = [C.c_void_p, C.POINTER(PkProblemDesc), _FP, _FP, _FP, _FP, _FP, C.c_int64, C.c_void_p]
     lib.pk_constraint_rows_batched.argtypes = [C.c_void_p, C.POINTER(PkProblemDesc), _FP, _FP, _FP, _FP, _FP, _FP, _FP, _FP, C.c_int64, C.c_void_p]
     lib.pk_task_terms_batched.argtypes = [C.c_void_p, C.POINTER(PkProblemDesc), C.c_int32, _FP, _FP, _FP, _FP, C.c_int64, C.c_void_p]
@@ -224,6 +226,7 @@ EXPORTED_SYMBOLS = [
     "pk_solve_ik_prepared",
     "pk_solve_ik_prepared_host",
     "pk_rollout_prepared",
+    "pk_rollout_trajectory_prepared",
     "pk_build_ik_batched",
     "pk_constraint_rows_batched",
     "pk_task_terms_batched",

@@ -12,13 +12,28 @@ launch through ``pk_solve_ik_prepared``.
 from __future__ import annotations
 
 import ctypes as C
-from typing import Iterable, Optional
+from typing import Iterable, NamedTuple, Optional
 
 import torch
 
 from . import _cabi
 from .engine import _addr, _stream, get_engine
 from .solve_ik import describe_problem
+
+
+class RolloutTrajectory(NamedTuple):
+    """Result of :meth:`BatchedIK.rollout_trajectory`.  ``q [B, nq]`` final configurations,
+    ``v [B, nv]`` velocity of the last step that ran, ``status [B]`` OR over the steps that ran;
+    the records (``None`` without ``record``) are step-major: ``q_traj [steps, B, nq]`` q after
+    each step, ``v_traj [steps, B, nv]`` velocity of each step, ``status_traj [steps, B]`` OR of
+    the statuses up to each step."""
+
+    q: torch.Tensor
+    v: torch.Tensor
+    status: torch.Tensor
+    q_traj: Optional[torch.Tensor]
+    v_traj: Optional[torch.Tensor]
+    status_traj: Optional[torch.Tensor]
 
 
 class BatchedIK:
@@ -143,3 +158,69 @@ class BatchedIK:
             _cabi.check(eng.lib.pk_rollout_prepared(eng.handle, self._handle, _addr(q), _addr(targets), int(steps),
                                                     _addr(q_out), _addr(v_out), _addr(status), B, _stream(eng.device)))
         return q_out, v_out, status
+
+    def rollout_trajectory(self, q: torch.Tensor, targets: Optional[torch.Tensor], steps: Optional[int] = None,
+                           record: bool = True, q_out: Optional[torch.Tensor] = None,
+                           v_out: Optional[torch.Tensor] = None,
+                           status: Optional[torch.Tensor] = None) -> RolloutTrajectory:
+        """``steps`` iterations of ``v = solve_ik(q, targets[s]); q = q (+) v dt`` in one launch:
+        the loop of ``examples/arm_ur5.py:65-86`` with a target that moves every step.
+
+        ``targets`` is ``[steps, B, target_stride]`` (one row per instance and step; a view is
+        fine as long as ``stride(2) == 1`` and ``stride(1) == target_stride``), or ``[B,
+        target_stride]`` / ``None`` with ``steps`` for the same rows every step.  With
+        ``record`` the configuration, velocity and status of every step come back too.  An
+        instance that fails a step (no solution, or outside its limits with ``safety_break``)
+        is frozen: its q stays, its later ``v_traj`` rows are zero and ``status_traj``
+        repeats.  The ``dq_prev`` words of ``AccelerationLimit`` / ``LowAccelerationTask`` are
+        read from each step's row as given.  Asynchronous on the current stream; no
+        allocation inside the library, so the call can be captured in a CUDA graph."""
+        eng = self.engine
+        B = q.shape[0]
+        S = self.target_stride
+        if targets is None:
+            if S > 0:
+                raise ValueError(f"this problem has per-instance targets ({S} floats per row): pass targets")
+            if steps is None:
+                raise ValueError("steps is required when targets is None")
+            target_step = 0
+        elif targets.dim() == 2:
+            if steps is None:
+                raise ValueError("steps is required with one targets row per instance")
+            if tuple(targets.shape) != (B, S):
+                raise ValueError(f"targets has shape {tuple(targets.shape)}, expected ({B}, {S})")
+            if S > 0 and (targets.stride(1) != 1 or targets.stride(0) != S):
+                raise ValueError("targets rows must be contiguous, target_stride floats apart")
+            target_step = 0
+        elif targets.dim() == 3:
+            if steps is None:
+                steps = targets.shape[0]
+            if targets.shape[0] != steps:
+                raise ValueError(f"targets holds {targets.shape[0]} steps, steps = {steps}")
+            if tuple(targets.shape[1:]) != (B, S):
+                raise ValueError(f"targets has shape {tuple(targets.shape)}, expected ({steps}, {B}, {S})")
+            if S > 0 and (targets.stride(2) != 1 or targets.stride(1) != S):
+                raise ValueError("targets[s] rows must be contiguous, target_stride floats apart "
+                                 f"(strides {tuple(targets.stride())})")
+            target_step = targets.stride(0) if steps > 1 else 0
+        else:
+            raise ValueError(f"targets must be [steps, B, {S}] or [B, {S}], got {tuple(targets.shape)}")
+        if targets is not None and targets.dtype != torch.float32:
+            raise ValueError(f"targets must be float32, got {targets.dtype}")
+        steps = int(steps)
+        if q_out is None:
+            q_out = torch.empty_like(q)
+        if v_out is None:
+            v_out = torch.empty((B, self.nv), device=eng.device, dtype=torch.float32)
+        if status is None:
+            status = torch.empty((B,), device=eng.device, dtype=torch.int32)
+        q_traj = v_traj = st_traj = None
+        if record and steps > 0:
+            q_traj = torch.empty((steps, B, self.nq), device=eng.device, dtype=torch.float32)
+            v_traj = torch.empty((steps, B, self.nv), device=eng.device, dtype=torch.float32)
+            st_traj = torch.empty((steps, B), device=eng.device, dtype=torch.int32)
+        with torch.cuda.device(eng.device):
+            _cabi.check(eng.lib.pk_rollout_trajectory_prepared(
+                eng.handle, self._handle, _addr(q), _addr(targets), int(target_step), steps, _addr(q_out),
+                _addr(v_out), _addr(status), _addr(q_traj), _addr(v_traj), _addr(st_traj), B, _stream(eng.device)))
+        return RolloutTrajectory(q_out, v_out, status, q_traj, v_traj, st_traj)

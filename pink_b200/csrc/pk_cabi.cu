@@ -357,12 +357,34 @@ __device__ __forceinline__ bool chain_copy_row(float* dst, const float* src, int
   return diff == 0u;
 }
 
+// Records of step s of a trajectory (thread-per-instance chain kernel); `frozen`: v row of zeros.
+template <int NJ>
+__device__ __forceinline__ void chain_record(const Trajectory& T, int s, int64_t B, int64_t i, const float (&qi)[NJ],
+                                             const float (&vi)[NJ], int st_all, bool frozen) {
+  const int64_t r = (int64_t)s * B + i;
+  if (T.q) {
+#pragma unroll
+    for (int k = 0; k < NJ; ++k) T.q[r * NJ + k] = qi[k];
+  }
+  if (T.v) {
+#pragma unroll
+    for (int k = 0; k < NJ; ++k) T.v[r * NJ + k] = frozen ? 0.f : vi[k];
+  }
+  if (T.status) T.status[r] = st_all;
+}
+
+// T: per-step targets and records of a trajectory call, read by the plain instantiation only.
+// The PDL protocol validates one copied targets row after the wait and stores nothing before
+// it, so it cannot cover K rows or per-step stores: trajectory calls with a step stride or
+// records always launch <NJ, NFT, false>.  Every step's row is read through load_se3_vec4,
+// which checks each address, so a step stride that is not a multiple of 4 floats takes the
+// scalar loads.
 template <int NJ, int NFT, bool PDL>
 __global__ void __launch_bounds__(128, 4)
     ik_chain_kernel(const __grid_constant__ ChainParams<NJ> P, const float* __restrict__ q,
                     const float* __restrict__ targets, float* __restrict__ v, int32_t* __restrict__ status,
                     int64_t B, int flags, int n_steps, float* __restrict__ q_out,
-                    const __grid_constant__ PeerOut peers) {
+                    const __grid_constant__ PeerOut peers, const __grid_constant__ Trajectory T) {
   if constexpr (PDL) pdl_launch_dependents();
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   peer_gate(peers);
@@ -402,13 +424,23 @@ __global__ void __launch_bounds__(128, 4)
     for (int step_no = 0; step_no < n_steps; ++step_no) {
       const bool frozen =
           (st_all & (PK_STATUS_NO_SOLUTION | PK_STATUS_NOT_POSDEF)) || ((st_all & PK_STATUS_OUT_OF_LIMITS) && P.safety_break);
-      if (frozen) break;
+      if (frozen) {
+        if constexpr (!PDL) {
+#pragma unroll 1
+          for (int s = step_no; s < n_steps; ++s) chain_record<NJ>(T, s, B, i, qi, vi, st_all, true);
+        }
+        break;
+      }
       int st;
       ik_step_chain<NJ, NFT>(P, qi, trow, vi, st, flags);
       st_all |= st & 0xff;
       if (n_steps > 1 || q_out) {
 #pragma unroll
         for (int k = 0; k < NJ; ++k) qi[k] = fmaf(vi[k], P.dt, qi[k]);  // 1-dof joints: q (+) v dt = q + v dt
+      }
+      if constexpr (!PDL) {
+        trow += T.target_step;
+        chain_record<NJ>(T, step_no, B, i, qi, vi, st_all, false);
       }
     }
     if constexpr (!PDL) {
@@ -495,6 +527,55 @@ __global__ void __launch_bounds__(64) ik_generic_kernel(const DevModel M, const 
   G.step(M, P, A.q + i * M.nq, A.targets ? A.targets + i * (int64_t)P.target_stride : nullptr, out);
 }
 
+// Records of step s of a trajectory from an instance's q / v rows (`n` threads from `lane`).
+__device__ __forceinline__ void record_rows(const Trajectory& T, int s, int64_t B, int64_t i, int nq, int nv,
+                                            const float* qrow, const float* vrow, int st_all, bool frozen,
+                                            int lane, int n) {
+  const int64_t r = (int64_t)s * B + i;
+  if (T.q)
+    for (int k = lane; k < nq; k += n) T.q[r * nq + k] = qrow[k];
+  if (T.v)
+    for (int k = lane; k < nv; k += n) T.v[r * nv + k] = frozen ? 0.f : vrow[k];
+  if (T.status && lane == 0) T.status[r] = st_all;
+}
+
+// Trajectory rollout of the general path in one launch: per thread, n_steps iterations of
+// Generic::step and q (+) v dt on the instance's q_out row in place, with the freeze rule of the
+// chain kernel (an instance that fails a step is frozen after it; status = OR over the steps
+// that ran).
+template <int NJMAX, int NVMAX>
+__global__ void __launch_bounds__(64)
+    ik_generic_rollout_kernel(const DevModel M, const __grid_constant__ DevProblem P, const float* q,
+                              const float* __restrict__ targets, int n_steps, float* q_out, float* __restrict__ v,
+                              int32_t* __restrict__ status, int64_t B, const __grid_constant__ Trajectory T) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= B) return;
+  const int nq = M.nq, nv = M.nv;
+  float* qrow = q_out + i * nq;
+  float* vrow = v + i * nv;
+  for (int k = 0; k < nq; ++k) qrow[k] = q[i * nq + k];
+  int32_t st = 0;
+  GenericOut out{};
+  out.v = vrow;
+  out.status = &st;
+  out.task_index = -1;
+  Generic<NJMAX, NVMAX> G;
+  int st_all = 0;
+  for (int s = 0; s < n_steps; ++s) {
+    const bool frozen =
+        (st_all & (PK_STATUS_NO_SOLUTION | PK_STATUS_NOT_POSDEF)) || ((st_all & PK_STATUS_OUT_OF_LIMITS) && P.safety_break);
+    if (frozen) {
+      record_rows(T, s, B, i, nq, nv, qrow, vrow, st_all, true, 0, 1);
+      continue;
+    }
+    G.step(M, P, qrow, targets ? targets + s * T.target_step + i * (int64_t)P.target_stride : nullptr, out);
+    st_all |= st;
+    integrate_configuration(nq, M.free_flyer, qrow, vrow, P.dt, qrow);
+    record_rows(T, s, B, i, nq, nv, qrow, vrow, st_all, false, 0, 1);
+  }
+  if (status) status[i] = st_all;
+}
+
 // Tree kernel: one instance per warp, per-instance state in the warp's slice of
 // dynamic shared memory (pk_tree.cuh).
 constexpr int kTreeWarpsPerBlock = 2;
@@ -521,10 +602,14 @@ __global__ void __launch_bounds__(32 * kTreeWarpsPerBlock, PK_TREE_MIN_BLOCKS)
 // per warp, the instance's q / v rows re-read by the warp that wrote them (they stay in
 // L1 / L2; the per-step launch pair and its two full passes over HBM are gone).  An instance
 // that fails a step (no solution / outside limits with safety_break) is frozen, as on chains.
+// T: per-step targets rows and records of a trajectory call (pk_rollout_trajectory_prepared); the
+// lanes store the q / v rows into the records after every step, and a frozen instance's warp
+// fills its remaining steps (q unchanged, v = 0, the same status).
 __global__ void __launch_bounds__(32 * kTreeWarpsPerBlock)
     ik_tree_rollout_kernel(const DevModel M, const __grid_constant__ DevProblem P, const __grid_constant__ TreePlan L,
                            const float* __restrict__ q, const float* __restrict__ targets, int n_steps,
-                           float* __restrict__ q_out, float* __restrict__ v, int32_t* __restrict__ status, int64_t B) {
+                           float* __restrict__ q_out, float* __restrict__ v, int32_t* __restrict__ status, int64_t B,
+                           const __grid_constant__ Trajectory T) {
   extern __shared__ __align__(16) float tree_smem[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int64_t i = (int64_t)blockIdx.x * kTreeWarpsPerBlock + warp;
@@ -535,17 +620,20 @@ __global__ void __launch_bounds__(32 * kTreeWarpsPerBlock)
   for (int k = lane; k < L.nq; k += 32) qrow[k] = q[i * L.nq + k];
   __syncwarp();
   int st_all = 0;
-  for (int s = 0; s < n_steps; ++s) {
+  int s = 0;
+  while (s < n_steps) {
     int32_t st = 0;
-    TreeStep::run(M, P, L, qrow, targets ? targets + i * (int64_t)L.stride : nullptr, W, vrow, &st);
+    TreeStep::run(M, P, L, qrow, targets ? targets + s * T.target_step + i * (int64_t)L.stride : nullptr, W, vrow, &st);
     __syncwarp();
     st = __shfl_sync(0xffffffffu, st, 0);  // run() reports through lane 0
     st_all |= st;
     const bool failed = (st & (PK_STATUS_NO_SOLUTION | PK_STATUS_NOT_POSDEF)) || ((st & PK_STATUS_OUT_OF_LIMITS) && P.safety_break);
-    if (failed) break;
-    if (lane == 0) integrate_configuration(L.nq, M.free_flyer, qrow, vrow, P.dt, qrow);
+    if (!failed && lane == 0) integrate_configuration(L.nq, M.free_flyer, qrow, vrow, P.dt, qrow);
     __syncwarp();
+    record_rows(T, s++, B, i, L.nq, L.nv, qrow, vrow, st_all, false, lane, 32);
+    if (failed) break;
   }
+  for (; s < n_steps; ++s) record_rows(T, s, B, i, L.nq, L.nv, qrow, vrow, st_all, true, lane, 32);
   if (status && lane == 0) status[i] = st_all;
 }
 
@@ -630,18 +718,25 @@ int launched() {
 }
 
 const pk::PeerOut kNoPeers{};
+const pk::Trajectory kNoTrajectory{};
+
+// a call the PDL instantiation of the chain kernel cannot run: per-step targets rows or records
+bool per_step(const pk::Trajectory& T) { return T.target_step != 0 || T.q || T.v || T.status; }
 
 template <int NJ, int NFT>
 int launch_chain(const pk::ChainParams<NJ>& C, bool pdl_row_fits, const float* q, const float* targets, float* v,
-                 int32_t* status, int64_t B, cudaStream_t stream, int n_steps, float* q_out, const pk::PeerOut& peers) {
+                 int32_t* status, int64_t B, cudaStream_t stream, int n_steps, float* q_out, const pk::PeerOut& peers,
+                 const pk::Trajectory& traj) {
   // A/B and probe switches (timing experiments; see scripts/ab.sh)
   static const int flags = (env_int("PK_CLOSED_FORM", 1) ? 0 : 1) | (env_int("PK_PROBE_SKIP_ROUNDS", 0) ? 2 : 0) |
                            (env_int("PK_CHAIN_FORCE_RECOMPUTE", 0) ? pk::kChainForceRecompute : 0);
   static const int block = env_int("PK_CHAIN_BLOCK", 128);
   const int64_t grid = (B + block - 1) / block;
   // PDL unless the fused peer gather is on (peer_gate and its flag protocol assume full stream
-  // order) or the targets row is longer than the kernel's copy of it
-  if (PK_CHAIN_PDL && peers.n == 0 && pdl_row_fits && !g_chain_pdl_rejected.load(std::memory_order_relaxed)) {
+  // order), the targets row is longer than the kernel's copy of it, or a trajectory call reads
+  // a row per step or stores records
+  if (PK_CHAIN_PDL && peers.n == 0 && pdl_row_fits && !per_step(traj) &&
+      !g_chain_pdl_rejected.load(std::memory_order_relaxed)) {
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3((unsigned)grid);
     cfg.blockDim = dim3(block);
@@ -652,14 +747,14 @@ int launch_chain(const pk::ChainParams<NJ>& C, bool pdl_row_fits, const float* q
     cfg.attrs = attr;
     cfg.numAttrs = 1;
     if (cudaLaunchKernelEx(&cfg, pk::ik_chain_kernel<NJ, NFT, true>, C, q, targets, v, status, B, flags, n_steps, q_out,
-                           peers) == cudaSuccess)
+                           peers, traj) == cudaSuccess)
       return launched();
     // a driver or capture mode that rejects the attribute: plain launches from now on
     cudaGetLastError();
     g_chain_pdl_rejected.store(true, std::memory_order_relaxed);
   }
   pk::ik_chain_kernel<NJ, NFT, false><<<(unsigned)grid, block, 0, stream>>>(C, q, targets, v, status, B, flags, n_steps,
-                                                                          q_out, peers);
+                                                                          q_out, peers, traj);
   return launched();
 }
 
@@ -670,6 +765,19 @@ int launch_generic(const PkModel* m, int size_class, const pk::DevProblem& P, co
   const int64_t grid = (B + block - 1) / block;
   pk::with_generic(size_class, [&](auto nj, auto nv) {
     pk::ik_generic_kernel<decltype(nj)::value, decltype(nv)::value><<<(unsigned)grid, block, 0, stream>>>(m->dev, P, A, B);
+  });
+  return launched();
+}
+
+// The general path's trajectory rollout: one launch of ik_generic_rollout_kernel
+int launch_generic_rollout(const PkModel* m, int size_class, const pk::DevProblem& P, const float* q,
+                           const float* targets, int n_steps, float* q_out, float* v, int32_t* status, int64_t B,
+                           cudaStream_t stream, const pk::Trajectory& traj) {
+  const int block = 64;
+  const int64_t grid = (B + block - 1) / block;
+  pk::with_generic(size_class, [&](auto nj, auto nv) {
+    pk::ik_generic_rollout_kernel<decltype(nj)::value, decltype(nv)::value>
+        <<<(unsigned)grid, block, 0, stream>>>(m->dev, P, q, targets, n_steps, q_out, v, status, B, traj);
   });
   return launched();
 }
@@ -790,9 +898,11 @@ int prepare_problem(const PkModel* m, const PkProblemDesc* desc, PkProblem* pr, 
 }
 
 // The chain kernels of a prepared chain problem; n_steps > 1 or q_out: closed-loop rollout.
-// `peers`: the fused gather epilogue, which lives in the thread-per-instance kernel.
+// `peers`: the fused gather epilogue, which lives in the thread-per-instance kernel.  `traj`:
+// per-step targets rows and records of a trajectory rollout.
 int launch_chain_prepared(const PkProblem& pr, const float* q, const float* targets, float* v, int32_t* status,
-                          int64_t B, cudaStream_t stream, int n_steps, float* q_out, const pk::PeerOut* peers) {
+                          int64_t B, cudaStream_t stream, int n_steps, float* q_out, const pk::PeerOut* peers,
+                          const pk::Trajectory& traj = kNoTrajectory) {
   return pk::with_nj(pr.sel.nj, [&](auto nj) {
     constexpr int NJ = decltype(nj)::value;
     return pk::with_nft(pr.sel.nft, [&](auto nft) {
@@ -803,12 +913,12 @@ int launch_chain_prepared(const PkProblem& pr, const float* q, const float* targ
           const auto& C = *reinterpret_cast<const pk::CoopParams<pk::CoopStep<NJ, NFT, L>::NJP>*>(pr.coop_params);
           const int64_t grid = (B * L + pk::kCoopThreads - 1) / pk::kCoopThreads;
           pk::ik_coop_kernel<NJ, NFT, L>
-              <<<(unsigned)grid, pk::kCoopThreads, 0, stream>>>(C, q, targets, v, status, B, n_steps, q_out);
+              <<<(unsigned)grid, pk::kCoopThreads, 0, stream>>>(C, q, targets, v, status, B, n_steps, q_out, traj);
           return launched();
         });
       }
       return launch_chain<NJ, NFT>(*reinterpret_cast<const pk::ChainParams<NJ>*>(pr.chain_params), pr.sel.pdl_row_fits,
-                                   q, targets, v, status, B, stream, n_steps, q_out, peers ? *peers : kNoPeers);
+                                   q, targets, v, status, B, stream, n_steps, q_out, peers ? *peers : kNoPeers, traj);
     });
   });
 }
@@ -1000,7 +1110,7 @@ extern "C" int pk_rollout_prepared(const PkModel* m, const PkProblem* pr, const 
     return launch_chain_prepared(*pr, q, targets, v, status, B, stream, n_steps, q_out, nullptr);
   if (pr->sel.path == pk::kPathTree)  // joint trees: the whole loop in one launch of the warp kernel
     return launch_tree(pk::ik_tree_rollout_kernel, g_tree_rollout_smem, m, pr->sel.plan, B, stream, m->dev, pr->P,
-                       pr->sel.plan, q, targets, n_steps, q_out, v, status, B);
+                       pr->sel.plan, q, targets, n_steps, q_out, v, status, B, kNoTrajectory);
   // other models: the same closed loop as separate launches (solve, then integrate in place)
   if (q_out != q) PK_CUDA(cudaMemcpyAsync(q_out, q, sizeof(float) * B * m->nq, cudaMemcpyDeviceToDevice, stream));
   for (int s = 0; s < n_steps; ++s) {
@@ -1008,6 +1118,28 @@ extern "C" int pk_rollout_prepared(const PkModel* m, const PkProblem* pr, const 
     if (pk_integrate_batched(m, q_out, v, pr->P.dt, q_out, B, stream)) return 1;
   }
   return 0;
+}
+
+extern "C" int pk_rollout_trajectory_prepared(const PkModel* m, const PkProblem* pr, const float* q,
+                                              const float* targets, int64_t target_step, int32_t n_steps,
+                                              float* q_out, float* v, int32_t* status, float* q_traj, float* v_traj,
+                                              int32_t* status_traj, int64_t B, void* stream_) {
+  if (check_common(m, q, B)) return 1;
+  if (!pr) return fail("null problem");
+  if (n_steps < 1) return fail("n_steps must be >= 1");
+  if (target_step < 0) return fail("negative target_step");
+  if (B > 0 && (!v || !q_out)) return fail("null v or q_out");
+  if (B > 0 && pr->P.target_stride > 0 && !targets) return fail("null targets");
+  if (B == 0) return 0;
+  cudaStream_t stream = (cudaStream_t)stream_;
+  const pk::Trajectory traj{target_step, q_traj, v_traj, status_traj};
+  if (pr->sel.path == pk::kPathChain)
+    return launch_chain_prepared(*pr, q, targets, v, status, B, stream, n_steps, q_out, nullptr, traj);
+  if (pr->sel.path == pk::kPathTree)
+    return launch_tree(pk::ik_tree_rollout_kernel, g_tree_rollout_smem, m, pr->sel.plan, B, stream, m->dev, pr->P,
+                       pr->sel.plan, q, targets, n_steps, q_out, v, status, B, traj);
+  return launch_generic_rollout(m, pr->sel.generic_class, pr->P, q, targets, n_steps, q_out, v, status, B, stream,
+                                traj);
 }
 
 extern "C" int pk_solve_ik_batched(const PkModel* m, const PkProblemDesc* prob, const float* q,

@@ -363,4 +363,14 @@ PK_HD void integrate_configuration(int nq, int free_flyer, const float* qi,
   for (int j = 0; j < nq - rq; ++j) o[rq + j] = fmaf(vi[rv + j], dt, qi[rq + j]);
 }
 
+// Per-step targets and records of a trajectory rollout (pk_rollout_trajectory_prepared); all
+// zero for the fixed-target rollout.  The records are step-major: the row of instance i at
+// step s is row s B + i.
+struct Trajectory {
+  int64_t target_step;  // floats from one step's targets rows to the next (0: the same rows)
+  float* q;             // [n_steps][B][nq] q after each step, or null
+  float* v;             // [n_steps][B][nv] velocity of each step (0 once frozen), or null
+  int32_t* status;      // [n_steps][B] OR of the statuses up to each step, or null
+};
+
 }  // namespace pk

@@ -5,11 +5,14 @@
 Builds pink_b200/csrc/pk_cabi.cu of git revision BASE_REV (default HEAD) and of the working
 tree with __graft_entry__.NVCC_FLAGS plus -Xptxas -v, in parallel, then compares for every
 kernel:
-  - the cuobjdump -sass listing, with the /*addr*/ comments stripped;
+  - the cuobjdump -sass listing, with the /*addr*/ comments stripped and whitespace collapsed;
   - ptxas' registers / barriers / shared and constant memory line and its stack frame / spill
     line.
-A refactor of the host code must leave every kernel identical.  Prints one line per kernel
-that differs and a summary; exits 1 on any difference.  Nothing is written to the tree: the
+A refactor of the host code must leave every kernel identical.  Kernels are matched by their
+demangled name with the parameter list removed, so a kernel that gained a parameter is compared
+with its old self ("signature changed").  Prints one line per kernel that differs, was added or
+was removed, with the ptxas lines and SASS instruction counts of both builds for the kernels
+that differ, then a summary; exits 1 on any difference.  Nothing is written to the tree: the
 builds go to a temporary directory (or DIR).
 """
 
@@ -44,7 +47,8 @@ def sass_by_kernel(so):
             name = m.group(1)
             kernels[name] = []
         elif name is not None:
-            kernels[name].append(ADDR.sub("", line).rstrip())
+            # whitespace collapsed: cuobjdump pads its columns to the widest line of the whole listing
+            kernels[name].append(" ".join(ADDR.sub("", line).split()))
     return kernels
 
 
@@ -57,6 +61,29 @@ def ptxas_by_kernel(log):
         elif name and ("stack frame" in line or "Used " in line):
             info[name].append(line.strip())
     return info
+
+
+def demangle(names):
+    out = subprocess.run(["cu++filt"], input="\n".join(names), capture_output=True, text=True).stdout.splitlines()
+    return dict(zip(names, out))
+
+
+def strip_params(demangled):
+    """`void f<6, 1, true>(A, B)` -> `f<6, 1, true>`: drop the trailing parameter list and the
+    return type."""
+    s = demangled.strip()
+    if s.endswith(")"):
+        depth = 0
+        for k in range(len(s) - 1, -1, -1):
+            depth += {")": 1, "(": -1}.get(s[k], 0)
+            if depth == 0:
+                s = s[:k]
+                break
+    return s[5:] if s.startswith("void ") else s
+
+
+def n_instructions(lines):
+    return sum(1 for line in lines if ";" in line and not line.startswith(("/*", ".")))
 
 
 def main():
@@ -80,24 +107,43 @@ def main():
             sys.exit(f"{tag} build failed, see {d}/ptxas.txt")
     sass = {tag: sass_by_kernel(so) for tag, (_, so, _) in builds.items()}
     ptxas = {tag: ptxas_by_kernel(os.path.join(d, "ptxas.txt")) for tag, (d, _, _) in builds.items()}
-    names = sorted(set(sass["base"]) | set(sass["tree"]))
-    differ = 0
-    for n in names:
+    # kernel key (name and template arguments) -> mangled name, per build
+    keyed = {}
+    for tag in ("base", "tree"):
+        dm = demangle(sorted(sass[tag]))
+        keyed[tag] = {strip_params(d): (m, d) for m, d in dm.items()}
+    keys = sorted(set(keyed["base"]) | set(keyed["tree"]))
+    differ = added = removed = 0
+    for key in keys:
+        if key not in keyed["base"]:
+            added += 1
+            print(f"ADDED: {key}")
+            continue
+        if key not in keyed["tree"]:
+            removed += 1
+            print(f"REMOVED: {key}")
+            continue
+        (mb, db), (mt, dt) = keyed["base"][key], keyed["tree"][key]
         problems = []
-        if sass["base"].get(n) != sass["tree"].get(n):
+        if sass["base"][mb] != sass["tree"][mt]:
             problems.append("sass")
-        if ptxas["base"].get(n) != ptxas["tree"].get(n):
+        if ptxas["base"].get(mb) != ptxas["tree"].get(mt):
             problems.append("ptxas")
+        sig = " (signature changed)" if db != dt else ""
         if problems:
             differ += 1
-            print(f"DIFFERS ({', '.join(problems)}): {n}")
+            print(f"DIFFERS ({', '.join(problems)}){sig}: {key}")
+            for tag, m in (("base", mb), ("tree", mt)):
+                print(f"    {tag}: {n_instructions(sass[tag][m])} instructions; " + " | ".join(ptxas[tag].get(m, [])))
+        elif sig:
+            print(f"IDENTICAL{sig}: {key}")
     counts = defaultdict(int)
-    demangled = subprocess.run(["cu++filt"], input="\n".join(names), capture_output=True, text=True).stdout
-    for line in demangled.splitlines():
-        counts[re.search(r"(\w+)[<(]", line).group(1)] += 1
-    print("kernels:", len(names), dict(sorted(counts.items())))
-    print(f"{len(names) - differ} identical, {differ} differ (builds in {out})")
-    sys.exit(1 if differ else 0)
+    for key in keyed["tree"]:
+        counts[re.match(r"(?:\w+::)*(\w+)", key).group(1)] += 1
+    print("kernels:", len(keyed["tree"]), dict(sorted(counts.items())))
+    same = len(keys) - differ - added - removed
+    print(f"{same} identical, {differ} differ, {added} added, {removed} removed (builds in {out})")
+    sys.exit(1 if differ or added or removed else 0)
 
 
 if __name__ == "__main__":
