@@ -260,6 +260,28 @@ int pk_rollout_trajectory_prepared(const PkModel* model, const PkProblem* proble
                                    float* q_traj, float* v_traj, int32_t* status_traj,
                                    int64_t B, void* stream);
 
+/* Solve to a tolerance (the loop of the reference's examples/inverse_kinematics_ur10.py:
+ * while err > stop_thres), per instance, with fixed targets (one row per instance, as
+ * pk_rollout_prepared).  err(q) = max over the tasks t of task_mask (bit t = problem task t)
+ * of |e_t(q)|_2, the unweighted, gain-free error of pk_task_terms_batched.  For s = 0, 1, ...:
+ * stop at q_s if err(q_s) <= tol or s == max_steps; else solve step s (the step
+ * pk_rollout_prepared takes), stop at q_s if it fails (NO_SOLUTION / NOT_POSDEF, or
+ * OUT_OF_LIMITS with safety_break), else q_{s+1} = q_s (+) v dt.
+ *   q_out[B][nq]  where the instance stopped (required; may alias q),
+ *   err[B]        err(q_out); an instance has converged iff err <= tol (a NaN never has),
+ *   steps[B]      solves that ran,
+ *   status[B]     OR of their statuses (0 if none ran); err, steps, status may be NULL.
+ * Joint-velocity-type tasks cannot be in the mask (their error does not depend on q);
+ * barriers and constraints act in every step but do not enter err.  In fp32 a pose
+ * resolves to about 1e-7, so a tol below about 1e-6 may run to max_steps.  One launch on
+ * every path (serial chains always take the thread-per-instance kernel, whatever
+ * PK_CHAIN_LANES says); no host synchronisation and no allocation, so the call can be
+ * captured in a CUDA graph.                                                              */
+int pk_converge_prepared(const PkModel* model, const PkProblem* problem,
+                         const float* q, const float* targets, uint32_t task_mask, float tol,
+                         int32_t max_steps, float* q_out, float* err, int32_t* steps,
+                         int32_t* status, int64_t B, void* stream);
+
 /* ---- multi-GPU: all-gather of v through NVLink peer memory (SURVEY.md section 8e) ----
  * One process per GPU; instances are independent, so the only exchange is the one
  * BASELINE north_star names: collecting v.  Instead of a collective after the kernel, the

@@ -36,6 +36,18 @@ class RolloutTrajectory(NamedTuple):
     status_traj: Optional[torch.Tensor]
 
 
+class Convergence(NamedTuple):
+    """Result of :meth:`BatchedIK.converge`: ``q [B, nq]`` where each instance stopped,
+    ``error [B]`` its error there, ``steps [B]`` the solves that ran, ``status [B]`` the OR of
+    their statuses (0 if none ran), ``converged [B]`` = ``error <= tol``."""
+
+    q: torch.Tensor
+    error: torch.Tensor
+    steps: torch.Tensor
+    status: torch.Tensor
+    converged: torch.Tensor
+
+
 class BatchedIK:
     """``solve_ik`` with the problem description frozen.
 
@@ -61,6 +73,7 @@ class BatchedIK:
             sizes = [d.shape[0] for d in (t._pk_describe(model)["target"] for t in tasks) if isinstance(d, torch.Tensor)]
             batch_size = sizes[0] if sizes else 1
         self.engine = get_engine(model, device)
+        self.tasks = tasks
         self.prob, parts, descs = describe_problem(model, batch_size, tasks, dt, damping, list(limits), safety_break,
                                                    barriers, constraints, collision_model)
         self.target_stride = int(self.prob.target_stride)
@@ -224,3 +237,66 @@ class BatchedIK:
                 eng.handle, self._handle, _addr(q), _addr(targets), int(target_step), steps, _addr(q_out),
                 _addr(v_out), _addr(status), _addr(q_traj), _addr(v_traj), _addr(st_traj), B, _stream(eng.device)))
         return RolloutTrajectory(q_out, v_out, status, q_traj, v_traj, st_traj)
+
+    def converge(self, q: torch.Tensor, targets: Optional[torch.Tensor], tasks: Iterable, tol: float,
+                 max_steps: int, q_out: Optional[torch.Tensor] = None, error: Optional[torch.Tensor] = None,
+                 steps: Optional[torch.Tensor] = None, status: Optional[torch.Tensor] = None) -> Convergence:
+        """Solve each instance to a tolerance in one launch: the loop of the reference's
+        ``examples/inverse_kinematics_ur10.py`` (``while norm(task.compute_error(c)) > thres``).
+
+        ``err(q)`` is the largest ``|task.compute_error(q)|`` (unweighted, gain-free) over
+        ``tasks``, which must be task objects given to the constructor.  For s = 0, 1, ...
+        an instance stops at ``q_s`` when ``err(q_s) <= tol`` or ``s == max_steps``; otherwise
+        it takes the step :meth:`rollout` takes, and stops at ``q_s`` if that step fails (no
+        solution, or outside its limits with ``safety_break``).  ``targets [B,
+        target_stride]`` are fixed for the whole loop; the ``dq_prev`` words of
+        ``AccelerationLimit`` / ``LowAccelerationTask`` are read from the row as given.
+        Barriers and constraints act in every step but are not part of the stopping test.
+
+        Poses resolve to about 1e-7 in fp32, so a ``tol`` below about 1e-6 may run to
+        ``max_steps``.  Asynchronous on the current stream; no allocation inside the library,
+        so the call can be captured in a CUDA graph.  ``q_out`` may be ``q``."""
+        eng = self.engine
+        B = q.shape[0]
+        S = self.target_stride
+        mask = 0
+        for t in tasks:
+            ks = [k for k, t0 in enumerate(self.tasks) if t0 is t]
+            if not ks:
+                raise ValueError(f"{t!r} is not one of the tasks this solver was built with")
+            mask |= 1 << ks[0]
+        if mask == 0:
+            raise ValueError("tasks is empty: the stopping test needs at least one task")
+        for k in range(len(self.tasks)):
+            if (mask >> k) & 1 and int(self.prob.tasks[k].type) == _cabi.PK_TASK_JOINT_VELOCITY:
+                raise ValueError(f"{self.tasks[k]!r}: the error of a joint-velocity task does not depend on q")
+        tol = float(tol)
+        if not (tol >= 0.0) or tol == float("inf"):
+            raise ValueError(f"tol must be finite and >= 0, got {tol}")
+        if int(max_steps) != max_steps or max_steps < 0:
+            raise ValueError(f"max_steps must be an integer >= 0, got {max_steps}")
+        if tuple(q.shape) != (B, self.nq) or q.dtype != torch.float32 or not q.is_contiguous():
+            raise ValueError(f"q must be a contiguous float32 [B, {self.nq}] tensor")
+        if targets is None:
+            if S > 0:
+                raise ValueError(f"this problem has per-instance targets ({S} floats per row): pass targets")
+        else:
+            if targets.dim() != 2 or tuple(targets.shape) != (B, S):
+                raise ValueError(f"targets has shape {tuple(targets.shape)}, expected ({B}, {S})")
+            if S > 0 and (targets.stride(1) != 1 or targets.stride(0) != S):
+                raise ValueError("targets rows must be contiguous, target_stride floats apart")
+            if targets.dtype != torch.float32:
+                raise ValueError(f"targets must be float32, got {targets.dtype}")
+        if q_out is None:
+            q_out = torch.empty_like(q)
+        if error is None:
+            error = torch.empty((B,), device=eng.device, dtype=torch.float32)
+        if steps is None:
+            steps = torch.empty((B,), device=eng.device, dtype=torch.int32)
+        if status is None:
+            status = torch.empty((B,), device=eng.device, dtype=torch.int32)
+        with torch.cuda.device(eng.device):
+            _cabi.check(eng.lib.pk_converge_prepared(eng.handle, self._handle, _addr(q), _addr(targets), mask, tol,
+                                                     int(max_steps), _addr(q_out), _addr(error), _addr(steps),
+                                                     _addr(status), B, _stream(eng.device)))
+        return Convergence(q_out, error, steps, status, error <= tol)

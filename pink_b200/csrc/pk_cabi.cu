@@ -516,6 +516,31 @@ __global__ void __launch_bounds__(128, 4)
   peer_count_kernel(peers);
 }
 
+// Solve to a tolerance on chains (pk_converge_prepared): converge_chain per thread, q in
+// registers.  A plain launch: no PDL, no peer epilogue, no records.  q_out may alias q (each
+// thread reads its row before it writes it).  emask: the task mask in chain slots
+// (chain_task_mask).
+template <int NJ, int NFT>
+__global__ void __launch_bounds__(128, 4)
+    ik_chain_converge_kernel(const __grid_constant__ ChainParams<NJ> P, const float* q,
+                             const float* __restrict__ targets, unsigned emask, float tol, int max_steps,
+                             float* q_out, float* __restrict__ err, int32_t* __restrict__ steps,
+                             int32_t* __restrict__ status, int64_t B) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= B) return;
+  float qi[NJ];
+#pragma unroll
+  for (int k = 0; k < NJ; ++k) qi[k] = q[i * NJ + k];
+  float e;
+  int n, st;
+  converge_chain<NJ, NFT>(P, qi, targets + i * (int64_t)P.target_stride, emask, tol, max_steps, e, n, st);
+#pragma unroll
+  for (int k = 0; k < NJ; ++k) q_out[i * NJ + k] = qi[k];
+  if (err) err[i] = e;
+  if (steps) steps[i] = n;
+  if (status) status[i] = st;
+}
+
 // General path: one instance per thread, per-thread arrays in local memory.
 template <int NJMAX, int NVMAX>
 __global__ void __launch_bounds__(64) ik_generic_kernel(const DevModel M, const __grid_constant__ DevProblem P,
@@ -574,6 +599,30 @@ __global__ void __launch_bounds__(64)
     record_rows(T, s, B, i, nq, nv, qrow, vrow, st_all, false, 0, 1);
   }
   if (status) status[i] = st_all;
+}
+
+// Solve to a tolerance on the general path (pk_converge_prepared): converge_generic per thread
+// on the instance's q_out row in place; v in local memory.
+template <int NJMAX, int NVMAX>
+__global__ void __launch_bounds__(64)
+    ik_generic_converge_kernel(const DevModel M, const __grid_constant__ DevProblem P, const float* q,
+                               const float* __restrict__ targets, unsigned mask, float tol, int max_steps, float* q_out,
+                               float* __restrict__ err, int32_t* __restrict__ steps, int32_t* __restrict__ status,
+                               int64_t B) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= B) return;
+  const int nq = M.nq;
+  float* qrow = q_out + i * nq;
+  for (int k = 0; k < nq; ++k) qrow[k] = q[i * nq + k];
+  float v[NVMAX];
+  Generic<NJMAX, NVMAX> G;
+  float e;
+  int n, st;
+  converge_generic(G, M, P, qrow, targets ? targets + i * (int64_t)P.target_stride : nullptr, v, mask, tol, max_steps,
+                   e, n, st);
+  if (err) err[i] = e;
+  if (steps) steps[i] = n;
+  if (status) status[i] = st;
 }
 
 // Tree kernel: one instance per warp, per-instance state in the warp's slice of
@@ -635,6 +684,33 @@ __global__ void __launch_bounds__(32 * kTreeWarpsPerBlock)
   }
   for (; s < n_steps; ++s) record_rows(T, s, B, i, L.nq, L.nv, qrow, vrow, st_all, true, lane, 32);
   if (status && lane == 0) status[i] = st_all;
+}
+
+// Solve to a tolerance on joint trees (pk_converge_prepared): TreeStep::converge per warp on
+// the instance's q_out row in place; the step's v at word o_v of the warp's workspace (the
+// plan's words include it).  The warp leaves its loop as soon as its instance stops.
+__global__ void __launch_bounds__(32 * kTreeWarpsPerBlock)
+    ik_tree_converge_kernel(const DevModel M, const __grid_constant__ DevProblem P, const __grid_constant__ TreePlan L,
+                            int o_v, const float* q, const float* __restrict__ targets, unsigned mask, float tol,
+                            int max_steps, float* q_out, float* __restrict__ err, int32_t* __restrict__ steps,
+                            int32_t* __restrict__ status, int64_t B) {
+  extern __shared__ __align__(16) float tree_smem[];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int64_t i = (int64_t)blockIdx.x * kTreeWarpsPerBlock + warp;
+  if (i >= B) return;
+  float* W = tree_smem + (size_t)warp * L.words;
+  float* qrow = q_out + i * L.nq;
+  for (int k = lane; k < L.nq; k += 32) qrow[k] = q[i * L.nq + k];
+  __syncwarp();
+  float e;
+  int n, st;
+  TreeStep::converge(M, P, L, qrow, targets ? targets + i * (int64_t)L.stride : nullptr, W, W + o_v, mask, tol,
+                     max_steps, e, n, st);
+  if (lane == 0) {
+    if (err) err[i] = e;
+    if (steps) steps[i] = n;
+    if (status) status[i] = st;
+  }
 }
 
 // q (+) v dt
@@ -788,7 +864,7 @@ struct SmemGrant {
   std::mutex mu;
   size_t bytes[64] = {};
 };
-SmemGrant g_tree_smem, g_tree_rollout_smem;
+SmemGrant g_tree_smem, g_tree_rollout_smem, g_tree_converge_smem;
 
 // A tree kernel: one instance per warp, `plan.words` floats of dynamic shared memory per warp.
 template <class... Params, class... Args>
@@ -1140,6 +1216,50 @@ extern "C" int pk_rollout_trajectory_prepared(const PkModel* m, const PkProblem*
                        pr->sel.plan, q, targets, n_steps, q_out, v, status, B, traj);
   return launch_generic_rollout(m, pr->sel.generic_class, pr->P, q, targets, n_steps, q_out, v, status, B, stream,
                                 traj);
+}
+
+extern "C" int pk_converge_prepared(const PkModel* m, const PkProblem* pr, const float* q, const float* targets,
+                                    uint32_t task_mask, float tol, int32_t max_steps, float* q_out, float* err,
+                                    int32_t* steps, int32_t* status, int64_t B, void* stream_) {
+  if (check_common(m, q, B)) return 1;
+  if (!pr) return fail("null problem");
+  const std::string aerr = pk::check_converge_args(pr->P, task_mask, tol, max_steps);
+  if (!aerr.empty()) return fail(aerr);
+  if (B > 0 && !q_out) return fail("null q_out");
+  if (B > 0 && pr->P.target_stride > 0 && !targets) return fail("null targets");
+  if (B == 0) return 0;
+  cudaStream_t stream = (cudaStream_t)stream_;
+  const pk::Selection& sel = pr->sel;
+  if (sel.path == pk::kPathChain) {
+    // always the thread-per-instance kernel: PK_CHAIN_LANES selects only the solve entries' variant
+    const unsigned emask = pk::chain_task_mask(pr->P, task_mask, sel.nft);
+    const int block = 128;
+    const int64_t grid = (B + block - 1) / block;
+    pk::with_nj(sel.nj, [&](auto nj) {
+      constexpr int NJ = decltype(nj)::value;
+      pk::with_nft(sel.nft, [&](auto nft) {
+        pk::ik_chain_converge_kernel<NJ, decltype(nft)::value><<<(unsigned)grid, block, 0, stream>>>(
+            *reinterpret_cast<const pk::ChainParams<NJ>*>(pr->chain_params), q, targets, emask, tol, max_steps, q_out,
+            err, steps, status, B);
+      });
+    });
+    return launched();
+  }
+  if (sel.path == pk::kPathTree) {
+    // the step's v lives in the warp's workspace, after the plan's words (kept 4-word aligned)
+    pk::TreePlan plan = sel.plan;
+    const int o_v = plan.words;
+    plan.words += (plan.nv + 3) & ~3;
+    return launch_tree(pk::ik_tree_converge_kernel, g_tree_converge_smem, m, plan, B, stream, m->dev, pr->P, plan, o_v,
+                       q, targets, task_mask, tol, (int)max_steps, q_out, err, steps, status, B);
+  }
+  const int block = 64;
+  const int64_t grid = (B + block - 1) / block;
+  pk::with_generic(sel.generic_class, [&](auto nj, auto nv) {
+    pk::ik_generic_converge_kernel<decltype(nj)::value, decltype(nv)::value><<<(unsigned)grid, block, 0, stream>>>(
+        m->dev, pr->P, q, targets, task_mask, tol, max_steps, q_out, err, steps, status, B);
+  });
+  return launched();
 }
 
 extern "C" int pk_solve_ik_batched(const PkModel* m, const PkProblemDesc* prob, const float* q,

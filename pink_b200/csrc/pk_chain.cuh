@@ -82,13 +82,20 @@ struct ChainStep {
 
   // Returns status bits; `skip` is set when the instance must not be solved
   // (outside limits with safety_break).
-  PK_HD int assemble(const ChainParams<NJ>& P, const float (&q)[NJ], const float* __restrict__ trow, bool& skip) {
+  // ERR (converge_chain): also store in *err the largest unweighted, gain-free |e_t|_2 of the
+  // tasks of `emask` in chain slots (bit k < NFT: ft[k], bit NFT: the posture task).  An
+  // instance outside its limits still runs the forward kinematics then, because its error is
+  // wanted too; it returns right after the task errors.
+  template <bool ERR = false>
+  PK_HD int assemble(const ChainParams<NJ>& P, const float (&q)[NJ], const float* __restrict__ trow, bool& skip,
+                     unsigned emask = 0u, float* err = nullptr) {
   int status = 0;
+  float emax = 0.f;
 #pragma unroll
   for (int j = 0; j < NJ; ++j)
     if (q[j] < P.chk_lo[j] || q[j] > P.chk_hi[j]) status |= PK_STATUS_OUT_OF_LIMITS;
   skip = status && P.safety_break;
-  if (skip) return status;
+  if (skip && !ERR) return status;
 
   // ---- forward kinematics: oMi[j] = oMi[j-1] X_j exp(S_j q_j) -----------------
   SE3f T = identity_se3();
@@ -143,6 +150,14 @@ struct ChainStep {
     Log3 L = log3(Tbt.R);
     float e[6];
     log6(Tbt, L, e);
+    if constexpr (ERR) {
+      if ((emask >> t) & 1u) {
+        float n2 = 0.f;
+#pragma unroll
+        for (int k = 0; k < 6; ++k) n2 = fmaf(e[k], e[k], n2);
+        emax = err_max(emax, sqrtf(n2));
+      }
+    }
     // J = -Jlog6(T_t^-1 T_b) bJ_b ;  log3(R^T) = -log3(R), same angle and coefficients
     SE3f Ttb;
 #pragma unroll
@@ -209,6 +224,11 @@ struct ChainStep {
       d[j] = dd;
       beta[j] = k * pe[j];
     }
+    if constexpr (ERR) {
+      if ((emask >> NFT) & 1u) emax = err_max(emax, sqrtf(se));
+      *err = emax;
+      if (skip) return status;
+    }
   }
 
   // ---- box rows ------------------------------------------------------------------
@@ -260,6 +280,48 @@ PK_HD void ik_step_chain(const ChainParams<NJ>& P, const float (&q)[NJ], const f
 #pragma unroll
   for (int j = 0; j < NJ; ++j) v[j] = finite ? x[j] * P.inv_dt : 0.f;
   status_out = status;
+}
+
+// Solve to a tolerance (pk_converge_prepared), one instance, q in registers.  For s = 0, 1, ...:
+// err(q_s) = the largest |e_t|_2 of the tasks of `emask` (chain slots, see assemble); stop at
+// q_s when err <= tol or s == max_steps; otherwise take the step ik_step_chain takes (its status
+// ORed into status_out), stop at q_s if the freeze rule of the rollouts fires, and move to
+// q_s (+) v dt.  On return q is where the instance stopped, err its error, steps the solves.
+template <int NJ, int NFT>
+PK_HD void converge_chain(const ChainParams<NJ>& P, float (&q)[NJ], const float* __restrict__ trow, unsigned emask,
+                          float tol, int max_steps, float& err, int& steps, int& status_out, int flags = 0) {
+  int st_all = 0;
+  int s = 0;
+#pragma unroll 1
+  for (;; ++s) {
+    ChainStep<NJ, NFT> C;
+    bool skip;
+    float e;
+    const int status = C.template assemble<true>(P, q, trow, skip, emask, &e);
+    err = e;
+    if (e <= tol || s == max_steps) break;
+    // the rest of ik_step_chain
+    int st = status;
+    float x[NJ];
+#pragma unroll
+    for (int j = 0; j < NJ; ++j) x[j] = 0.f;
+    if (!skip && !(st & PK_STATUS_NO_SOLUTION))
+      st |= BoxLSQChol<6 * NFT, NJ>::run(C.A, C.b, C.d, C.beta, C.lo, C.hi, x, flags);
+    float sum = 0.f;
+#pragma unroll
+    for (int j = 0; j < NJ; ++j) sum += x[j];
+    const bool finite = fabsf(sum) < 3.0e38f;
+    if (!finite) st |= PK_STATUS_NO_SOLUTION;
+    st_all |= st & 0xff;
+    if (step_failed(st_all, P.safety_break)) {
+      ++s;
+      break;
+    }
+#pragma unroll
+    for (int k = 0; k < NJ; ++k) q[k] = fmaf(finite ? x[k] * P.inv_dt : 0.f, P.dt, q[k]);  // q (+) v dt = q + v dt
+  }
+  steps = s;
+  status_out = st_all;
 }
 
 }  // namespace pk

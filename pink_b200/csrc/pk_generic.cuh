@@ -445,7 +445,11 @@ struct Generic {
   }
 
   // One step. `q` [nq], `trow` per-instance targets.
-  PK_HD void step(const DevModel& M, const DevProblem& P, const float* q, const float* trow, const GenericOut& out) {
+  // ERR (converge_generic): also the stop test `ct` on the task errors, made before the QP; a
+  // step that stops there writes only *out.status (and ct).
+  template <bool ERR = false>
+  PK_HD void step(const DevModel& M, const DevProblem& P, const float* q, const float* trow, const GenericOut& out,
+                  ConvergeTest* ct = nullptr) {
     const int nv = M.nv;
     const int rq = M.free_flyer ? 7 : 0;
     const int rv = M.free_flyer ? 6 : 0;
@@ -493,6 +497,7 @@ struct Generic {
     int K = 0;
     float diag = P.damping;
     float Jw[6][NVMAX];
+    float emax = 0.f;  // ERR: largest |e_t|_2 of the tasks of ct->mask
 
     for (int t = 0; t < P.ntasks; ++t) {
       const DevTask& Kt = P.tasks[t];
@@ -510,6 +515,9 @@ struct Generic {
           if (want && out.e) out.e[i - rv] = e;
         }
         diag = fmaf(Kt.lm * Kt.gain * Kt.gain * w2, se, diag);
+        if constexpr (ERR) {
+          if ((ct->mask >> t) & 1u) emax = err_max(emax, sqrtf(se));
+        }
         if (want && out.J)
           for (int r = 0; r < nv - rv; ++r)
             for (int i = 0; i < nv; ++i) out.J[r * nv + i] = (i == r + rv) ? 1.f : 0.f;
@@ -517,6 +525,13 @@ struct Generic {
       }
       float e[6];
       const int k = task_rows(M, P, Kt, q, tgt, e, Jw);
+      if constexpr (ERR) {
+        if ((ct->mask >> t) & 1u) {
+          float n2 = 0.f;
+          for (int r = 0; r < k; ++r) n2 = fmaf(e[r], e[r], n2);
+          emax = err_max(emax, sqrtf(n2));
+        }
+      }
       if (want) {
         if (out.e)
           for (int r = 0; r < k; ++r) out.e[r] = e[r];
@@ -538,6 +553,15 @@ struct Generic {
       diag = fmaf(Kt.lm, mu, diag);
     }
     if (K > kGenericMaxRows) { status |= PK_STATUS_NOT_POSDEF; K = kGenericMaxRows; }
+    if constexpr (ERR) {
+      ct->err = emax;
+      ct->stop = emax <= ct->tol || ct->last;
+      ct->status = status;
+      if (ct->stop) {
+        if (out.status) *out.status = status;
+        return;
+      }
+    }
 
     // box of all +-e_i rows: configuration and velocity limits ...
     float lo[NVMAX], hi[NVMAX];
@@ -707,5 +731,35 @@ struct Generic {
     if (out.status) *out.status = status;
   }
 };
+
+// Solve to a tolerance (pk_converge_prepared), one instance on the general path; the loop of
+// converge_chain (pk_chain.cuh) with Generic::step.  q [nq]: in q_0, out where the instance
+// stopped (updated in place); v [nv]: scratch.
+template <int NJMAX, int NVMAX>
+PK_HD void converge_generic(Generic<NJMAX, NVMAX>& G, const DevModel& M, const DevProblem& P, float* q,
+                            const float* trow, float* v, unsigned mask, float tol, int max_steps, float& err,
+                            int& steps, int& status_out) {
+  int32_t st = 0;
+  GenericOut out{};
+  out.v = v;
+  out.status = &st;
+  out.task_index = -1;
+  int st_all = 0;
+  int s = 0;
+  for (;; ++s) {
+    ConvergeTest ct{mask, tol, s == max_steps, 0.f, false, 0};
+    G.template step<true>(M, P, q, trow, out, &ct);
+    err = ct.err;
+    if (ct.stop) break;
+    st_all |= st;
+    if (step_failed(st_all, P.safety_break)) {
+      ++s;
+      break;
+    }
+    integrate_configuration(M.nq, M.free_flyer, q, v, P.dt, q);
+  }
+  steps = s;
+  status_out = st_all;
+}
 
 }  // namespace pk

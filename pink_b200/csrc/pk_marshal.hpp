@@ -178,6 +178,19 @@ inline int task_terms_rows(const HostModel& m, const DevTask& d) {
   return is_diag_task(d.type) ? m.nv - (m.free_flyer ? 6 : 0) : task_row_count(m, d);
 }
 
+// Arguments of pk_converge_prepared; "" when valid.  Joint-velocity-type tasks cannot be in the
+// mask: their error does not depend on q.
+inline std::string check_converge_args(const DevProblem& P, uint32_t mask, float tol, int max_steps) {
+  if (mask == 0u) return "empty task mask";
+  if (P.ntasks < 32 && (mask >> P.ntasks) != 0u) return "task mask has bits at or above the number of tasks";
+  for (int t = 0; t < P.ntasks; ++t)
+    if (((mask >> t) & 1u) && P.tasks[t].type == PK_TASK_JOINT_VELOCITY)
+      return "a joint-velocity task (JointVelocityTask, DampingTask, LowAccelerationTask) cannot be in the task mask";
+  if (!(tol >= 0.f) || !std::isfinite(tol)) return "tol must be finite and >= 0";
+  if (max_steps < 0) return "max_steps must be >= 0";
+  return "";
+}
+
 // Problem of the forward-kinematics and frame-Jacobian exports: no tasks, no limits.
 inline DevProblem kinematics_problem() {
   DevProblem P;

@@ -373,4 +373,26 @@ struct Trajectory {
   int32_t* status;      // [n_steps][B] OR of the statuses up to each step, or null
 };
 
+// The freeze rule of the rollouts: an instance whose statuses so far have one of these bits
+// takes no further step.
+PK_HD bool step_failed(int st_all, int safety_break) {
+  return (st_all & (PK_STATUS_NO_SOLUTION | PK_STATUS_NOT_POSDEF)) || ((st_all & PK_STATUS_OUT_OF_LIMITS) && safety_break);
+}
+
+// max(m, n) that keeps a NaN: a NaN task error makes the whole error NaN (never <= tol).
+PK_HD float err_max(float m, float n) { return (n > m || n != n) ? n : m; }
+
+// Stop test of one step of a converge loop (pk_converge_prepared), for the step bodies that
+// take it: in mask (bit t: task t of the problem), tol, last (s == max_steps); out the error,
+// max over the tasks of mask of |e_t|_2 (unweighted, gain-free), whether the loop stops here
+// (the step then returns before its QP), and the step's status (the same on every lane).
+struct ConvergeTest {
+  unsigned mask;
+  float tol;
+  bool last;
+  float err;
+  bool stop;
+  int status;
+};
+
 }  // namespace pk

@@ -56,6 +56,23 @@ inline Selection select_kernel(const HostModel& m, const DevProblem& P, const Ho
   return s;
 }
 
+// A task mask of pk_converge_prepared (bit t: P.tasks[t]) in the chain kernels' slots: the frame
+// tasks are compacted into ft[] in task order (bit k: ft[k]), the posture task is bit nft.
+inline unsigned chain_task_mask(const DevProblem& P, unsigned mask, int nft) {
+  unsigned out = 0u;
+  int f = 0;
+  for (int t = 0; t < P.ntasks; ++t) {
+    const bool on = (mask >> t) & 1u;
+    if (P.tasks[t].type == PK_TASK_FRAME) {
+      if (on) out |= 1u << f;
+      ++f;
+    } else if (on) {
+      out |= 1u << nft;
+    }
+  }
+  return out;
+}
+
 // f(std::integral_constant<int, N>) for the run-time value: the chain kernels' joint count
 // (2..7, chain_eligible), frame-task count (0..2), sub-warp lanes (a coop_has_variant), the
 // general path's <NJMAX, NVMAX>.

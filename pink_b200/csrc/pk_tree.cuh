@@ -627,8 +627,13 @@ struct TreeStep {
   }
 
   // ---- the whole step ----------------------------------------------------------------
+  // ERR (converge): also the stop test `ct` on the task errors, reduced across the warp and made
+  // before the rows of A; a step that stops there, or whose instance is outside its limits with
+  // safety_break, returns with v = 0.  ct->status is the step's status on every lane.
+  template <bool ERR = false>
   static PK_HD void run(const DevModel& M, const DevProblem& P, const TreePlan& L, const float* __restrict__ qg,
-                        const float* __restrict__ tg, float* W, float* __restrict__ vg, int32_t* status_out) {
+                        const float* __restrict__ tg, float* W, float* __restrict__ vg, int32_t* status_out,
+                        ConvergeTest* ct = nullptr) {
     const int nj = L.nj, nv = L.nv, rq = L.rq, rv = L.rv;
     float* qs = W + L.o_q;
     float* ts = W + L.o_t;
@@ -653,7 +658,7 @@ struct TreeStep {
       PK_WSYNC();
       if (lane_or(bad)) status |= PK_STATUS_OUT_OF_LIMITS;
     }
-    if (status && P.safety_break) {
+    if (!ERR && status && P.safety_break) {
       PK_LANES(l) {
         #pragma unroll 1
         for (int i = l; i < nv; i += 32) vg[i] = 0.f;
@@ -782,6 +787,46 @@ struct TreeStep {
       }
     }
     PK_WSYNC();
+    if constexpr (ERR) {
+      // the stop test: |e_t|_2 of the selected tasks, the diagonal ones summed across the lanes
+      float emax = 0.f;
+      #pragma unroll 1
+      for (int t = 0; t < P.ntasks; ++t) {
+        if (!((ct->mask >> t) & 1u)) continue;
+        const DevTask& Kt = P.tasks[t];
+        float n2 = 0.f;
+        if (is_diag_task(Kt.type)) {
+          const float* tgt = Kt.tgt_shared ? (P.shared + Kt.tgt_off) : (ts + Kt.tgt_off);
+          LaneVar<float> part;
+          PK_LANES(l) {
+            float s = 0.f;
+            #pragma unroll 1
+            for (int i = rv + l; i < nv; i += 32) {
+              const float e = diag_task_error(Kt.type, qs, tgt, i, rq, rv);
+              s = fmaf(e, e, s);
+            }
+            part[l] = s;
+          }
+          n2 = lane_sum(part);
+        } else {
+          const float* F = W + L.o_tf + kTreeTaskWords * t;
+          const int k = (Kt.type == PK_TASK_COM) ? 3 : (Kt.type == PK_TASK_LINEAR ? Kt.rows : 6);
+          #pragma unroll 1
+          for (int r = 0; r < k; ++r) n2 = fmaf(F[30 + r], F[30 + r], n2);
+        }
+        emax = err_max(emax, sqrtf(n2));
+      }
+      ct->err = emax;
+      ct->stop = emax <= ct->tol || ct->last;
+      ct->status = status;
+      if (ct->stop || (status && P.safety_break)) {
+        PK_LANES(l) {
+          #pragma unroll 1
+          for (int i = l; i < nv; i += 32) vg[i] = 0.f;
+        }
+        return;
+      }
+    }
     // ---- rows of A (column-parallel), b, diagonal terms -----------------------------------
     float diag = P.damping;
     int erow = 0;  // next equality row
@@ -1122,6 +1167,37 @@ struct TreeStep {
       for (int i = l; i < nv; i += 32) vg[i] = W[L.o_x + i] * P.inv_dt;
       if (l == 0 && status_out) *status_out = status;
     }
+    if constexpr (ERR) ct->status = status;
+  }
+
+  // Solve to a tolerance (pk_converge_prepared), one instance per warp; the loop of
+  // converge_chain (pk_chain.cuh) with run<true>.  qg [nq]: in q_0, out where the instance stopped
+  // (updated in place by lane 0); vg [nv]: scratch.  err, steps and status are the same on every
+  // lane, so the warp leaves the loop together.
+  static PK_HD void converge(const DevModel& M, const DevProblem& P, const TreePlan& L, float* qg, const float* tg,
+                             float* W, float* vg, unsigned mask, float tol, int max_steps, float& err, int& steps,
+                             int& status_out) {
+    int st_all = 0;
+    int s = 0;
+    #pragma unroll 1
+    for (;; ++s) {
+      ConvergeTest ct{mask, tol, s == max_steps, 0.f, false, 0};
+      run<true>(M, P, L, qg, tg, W, vg, nullptr, &ct);
+      PK_WSYNC();
+      err = ct.err;
+      if (ct.stop) break;
+      st_all |= ct.status;
+      if (step_failed(st_all, P.safety_break)) {
+        ++s;
+        break;
+      }
+      PK_LANES(l) {
+        if (l == 0) integrate_configuration(L.nq, M.free_flyer, qg, vg, P.dt, qg);
+      }
+      PK_WSYNC();
+    }
+    steps = s;
+    status_out = st_all;
   }
 };
 
