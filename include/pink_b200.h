@@ -282,6 +282,27 @@ int pk_converge_prepared(const PkModel* model, const PkProblem* problem,
                          int32_t max_steps, float* q_out, float* err, int32_t* steps,
                          int32_t* status, int64_t B, void* stream);
 
+/* Multi-start solve to a tolerance: target b is solved from the num_seeds = S seeds
+ * q_seeds[b][j] (row b*S + j of q_seeds[B*S][nq], only read) with the one targets row b
+ * (targets[B][target_stride]).  The S seeds advance in lockstep rounds s = 0, 1, ...: each seed
+ * that has not failed computes err(q_s) of pk_converge_prepared; the group stops when some seed
+ * has err <= tol, s == max_steps, or every seed has failed; otherwise every seed that has not
+ * failed takes the pk_converge_prepared step, and a seed whose step fails keeps q_s and its
+ * error.  The winner is the seed with the smallest error at the stopping round (a NaN counts as
+ * +inf, ties go to the lowest index).  Per target:
+ *   q_out[B][nq]  the winner's configuration (required; must not overlap q_seeds),
+ *   err[B]        its error, seed[B] its index, steps[B] the rounds the group ran,
+ *   status[B]     the OR of the winner's step statuses (0 if none ran); err, seed, steps,
+ *                 status may be NULL.
+ * S is 1, 2, 4, 8, 16 or 32; on the tree kernel S <= 8 and the S warp workspaces must fit one
+ * CTA's shared memory.  With S = 1 the outputs equal pk_converge_prepared's.  One launch, no
+ * host synchronisation and no allocation, so the call can be captured in a CUDA graph.      */
+int pk_converge_multistart_prepared(const PkModel* model, const PkProblem* problem,
+                                    const float* q_seeds, int32_t num_seeds, const float* targets,
+                                    uint32_t task_mask, float tol, int32_t max_steps, float* q_out,
+                                    float* err, int32_t* seed, int32_t* steps, int32_t* status,
+                                    int64_t B, void* stream);
+
 /* ---- multi-GPU: all-gather of v through NVLink peer memory (SURVEY.md section 8e) ----
  * One process per GPU; instances are independent, so the only exchange is the one
  * BASELINE north_star names: collecting v.  Instead of a collective after the kernel, the

@@ -196,6 +196,8 @@ def declare(lib: C.CDLL, prefix: str = "pk_") -> None:
                                                    _FP, _FP, _FP, C.c_int64, C.c_void_p]
     lib.pk_converge_prepared.argtypes = [C.c_void_p, C.c_void_p, _FP, _FP, C.c_uint32, C.c_float, C.c_int32, _FP, _FP,
                                          _FP, _FP, C.c_int64, C.c_void_p]
+    lib.pk_converge_multistart_prepared.argtypes = [C.c_void_p, C.c_void_p, _FP, C.c_int32, _FP, C.c_uint32, C.c_float,
+                                                    C.c_int32, _FP, _FP, _FP, _FP, _FP, C.c_int64, C.c_void_p]
     lib.pk_build_ik_batched.argtypes = [C.c_void_p, C.POINTER(PkProblemDesc), _FP, _FP, _FP, _FP, _FP, C.c_int64, C.c_void_p]
     lib.pk_constraint_rows_batched.argtypes = [C.c_void_p, C.POINTER(PkProblemDesc), _FP, _FP, _FP, _FP, _FP, _FP, _FP, _FP, C.c_int64, C.c_void_p]
     lib.pk_task_terms_batched.argtypes = [C.c_void_p, C.POINTER(PkProblemDesc), C.c_int32, _FP, _FP, _FP, _FP, C.c_int64, C.c_void_p]
@@ -230,6 +232,7 @@ EXPORTED_SYMBOLS = [
     "pk_rollout_prepared",
     "pk_rollout_trajectory_prepared",
     "pk_converge_prepared",
+    "pk_converge_multistart_prepared",
     "pk_build_ik_batched",
     "pk_constraint_rows_batched",
     "pk_task_terms_batched",

@@ -48,6 +48,23 @@ class Convergence(NamedTuple):
     converged: torch.Tensor
 
 
+class MultistartConvergence(NamedTuple):
+    """Result of :meth:`BatchedIK.converge_multistart`, per target: ``q [B, nq]`` the winning
+    seed's configuration, ``error [B]`` its error, ``seed [B]`` (int32) its index, ``steps [B]``
+    the rounds the group ran, ``status [B]`` the OR of the winner's step statuses (0 if it ran
+    none), ``converged [B]`` = ``error <= tol``."""
+
+    q: torch.Tensor
+    error: torch.Tensor
+    seed: torch.Tensor
+    steps: torch.Tensor
+    status: torch.Tensor
+    converged: torch.Tensor
+
+
+SEED_COUNTS = (1, 2, 4, 8, 16, 32)
+
+
 class BatchedIK:
     """``solve_ik`` with the problem description frozen.
 
@@ -73,6 +90,7 @@ class BatchedIK:
             sizes = [d.shape[0] for d in (t._pk_describe(model)["target"] for t in tasks) if isinstance(d, torch.Tensor)]
             batch_size = sizes[0] if sizes else 1
         self.engine = get_engine(model, device)
+        self.model = model
         self.tasks = tasks
         self.prob, parts, descs = describe_problem(model, batch_size, tasks, dt, damping, list(limits), safety_break,
                                                    barriers, constraints, collision_model)
@@ -258,7 +276,26 @@ class BatchedIK:
         so the call can be captured in a CUDA graph.  ``q_out`` may be ``q``."""
         eng = self.engine
         B = q.shape[0]
-        S = self.target_stride
+        mask, tol = self._stop_test(tasks, tol, max_steps)
+        if tuple(q.shape) != (B, self.nq) or q.dtype != torch.float32 or not q.is_contiguous():
+            raise ValueError(f"q must be a contiguous float32 [B, {self.nq}] tensor")
+        self._check_fixed_targets(targets, B)
+        if q_out is None:
+            q_out = torch.empty_like(q)
+        if error is None:
+            error = torch.empty((B,), device=eng.device, dtype=torch.float32)
+        if steps is None:
+            steps = torch.empty((B,), device=eng.device, dtype=torch.int32)
+        if status is None:
+            status = torch.empty((B,), device=eng.device, dtype=torch.int32)
+        with torch.cuda.device(eng.device):
+            _cabi.check(eng.lib.pk_converge_prepared(eng.handle, self._handle, _addr(q), _addr(targets), mask, tol,
+                                                     int(max_steps), _addr(q_out), _addr(error), _addr(steps),
+                                                     _addr(status), B, _stream(eng.device)))
+        return Convergence(q_out, error, steps, status, error <= tol)
+
+    def _stop_test(self, tasks: Iterable, tol: float, max_steps: int):
+        """The task mask and tol of :meth:`converge` / :meth:`converge_multistart`, validated."""
         mask = 0
         for t in tasks:
             ks = [k for k, t0 in enumerate(self.tasks) if t0 is t]
@@ -275,8 +312,11 @@ class BatchedIK:
             raise ValueError(f"tol must be finite and >= 0, got {tol}")
         if int(max_steps) != max_steps or max_steps < 0:
             raise ValueError(f"max_steps must be an integer >= 0, got {max_steps}")
-        if tuple(q.shape) != (B, self.nq) or q.dtype != torch.float32 or not q.is_contiguous():
-            raise ValueError(f"q must be a contiguous float32 [B, {self.nq}] tensor")
+        return mask, tol
+
+    def _check_fixed_targets(self, targets: Optional[torch.Tensor], B: int) -> None:
+        """One fixed targets row per instance (or target), ``[B, target_stride]``."""
+        S = self.target_stride
         if targets is None:
             if S > 0:
                 raise ValueError(f"this problem has per-instance targets ({S} floats per row): pass targets")
@@ -287,16 +327,98 @@ class BatchedIK:
                 raise ValueError("targets rows must be contiguous, target_stride floats apart")
             if targets.dtype != torch.float32:
                 raise ValueError(f"targets must be float32, got {targets.dtype}")
+
+    def converge_multistart(self, q_seeds: torch.Tensor, targets: Optional[torch.Tensor], tasks: Iterable, tol: float,
+                            max_steps: int, q_out: Optional[torch.Tensor] = None, error: Optional[torch.Tensor] = None,
+                            seed: Optional[torch.Tensor] = None, steps: Optional[torch.Tensor] = None,
+                            status: Optional[torch.Tensor] = None) -> MultistartConvergence:
+        """Solve each target to a tolerance from several seeds in one launch, stopping a target as
+        soon as one of its seeds converges.
+
+        ``q_seeds [B, S, nq]``: S start configurations per target (:meth:`sample_seeds` makes
+        them), S one of 1, 2, 4, 8, 16, 32 (at most 8 on the tree kernel, whose S warp
+        workspaces must also fit one CTA's shared memory).  ``targets [B, target_stride]``: one
+        row per target, shared by its seeds.  ``tasks``, ``tol`` and ``max_steps`` as
+        :meth:`converge`.  The S seeds advance in lockstep rounds: in round s every seed that
+        has not failed computes ``err(q_s)``; the group stops when some seed has ``err <= tol``,
+        ``s == max_steps``, or every seed has failed; otherwise every seed that has not failed
+        takes the :meth:`converge` step, and a seed whose step fails keeps ``q_s`` and its error.
+        The winner is the seed with the smallest error at the stopping round (NaN counts as
+        +inf, ties go to the lowest index).
+
+        With S = 1 the result equals :meth:`converge`'s.  With seed 0 the caller's start, every
+        target :meth:`converge` solves from it is solved here too, in at most as many steps.
+        Asynchronous on the current stream; no allocation inside the library, so the call can
+        be captured in a CUDA graph.  ``q_seeds`` is only read and must not overlap ``q_out``."""
+        eng = self.engine
+        mask, tol = self._stop_test(tasks, tol, max_steps)
+        if (q_seeds.dim() != 3 or q_seeds.shape[2] != self.nq or q_seeds.dtype != torch.float32
+                or not q_seeds.is_contiguous()):
+            raise ValueError(f"q_seeds must be a contiguous float32 [B, S, {self.nq}] tensor")
+        B, S = int(q_seeds.shape[0]), int(q_seeds.shape[1])
+        if S not in SEED_COUNTS:
+            raise ValueError(f"the number of seeds must be one of {SEED_COUNTS}, got {S}")
+        self._check_fixed_targets(targets, B)
+        lib = eng.lib
+        # the path-dependent limits on S (the tree kernel's): the library validates a call with no
+        # targets without launching anything
+        if lib.pk_converge_multistart_prepared(eng.handle, self._handle, None, S, None, mask, tol, int(max_steps),
+                                               None, None, None, None, None, 0, None):
+            raise ValueError("pink_b200: " + lib.pk_last_error().decode("utf-8", "replace"))
         if q_out is None:
-            q_out = torch.empty_like(q)
+            q_out = torch.empty((B, self.nq), device=eng.device, dtype=torch.float32)
         if error is None:
             error = torch.empty((B,), device=eng.device, dtype=torch.float32)
+        if seed is None:
+            seed = torch.empty((B,), device=eng.device, dtype=torch.int32)
         if steps is None:
             steps = torch.empty((B,), device=eng.device, dtype=torch.int32)
         if status is None:
             status = torch.empty((B,), device=eng.device, dtype=torch.int32)
         with torch.cuda.device(eng.device):
-            _cabi.check(eng.lib.pk_converge_prepared(eng.handle, self._handle, _addr(q), _addr(targets), mask, tol,
-                                                     int(max_steps), _addr(q_out), _addr(error), _addr(steps),
-                                                     _addr(status), B, _stream(eng.device)))
-        return Convergence(q_out, error, steps, status, error <= tol)
+            _cabi.check(lib.pk_converge_multistart_prepared(
+                eng.handle, self._handle, _addr(q_seeds), S, _addr(targets), mask, tol, int(max_steps), _addr(q_out),
+                _addr(error), _addr(seed), _addr(steps), _addr(status), B, _stream(eng.device)))
+        return MultistartConvergence(q_out, error, seed, steps, status, error <= tol)
+
+    def sample_seeds(self, q: torch.Tensor, num_seeds: int, generator: Optional[torch.Generator] = None) -> torch.Tensor:
+        """Seeds for :meth:`converge_multistart`: ``q [B, nq]`` -> ``[B, num_seeds, nq]``.
+
+        Seed 0 is ``q``.  In the other seeds, each coordinate with finite lower and upper limits
+        is drawn uniformly strictly inside them; a revolute coordinate without limits (URDF
+        ``continuous``) is drawn in [-pi, pi]; the other coordinates (unbounded prismatic
+        joints, the free-flyer root) are copied from ``q``.  Plain torch on ``q``'s device."""
+        return sample_seeds(self.model, q, num_seeds, generator)
+
+
+def sample_seeds(model, q: torch.Tensor, num_seeds: int, generator: Optional[torch.Generator] = None) -> torch.Tensor:
+    """:meth:`BatchedIK.sample_seeds` for a model."""
+    import math
+
+    import numpy as np
+
+    if q.dim() != 2 or q.shape[1] != model.nq:
+        raise ValueError(f"q must be a [B, {model.nq}] tensor")
+    if int(num_seeds) != num_seeds or num_seeds < 1:
+        raise ValueError(f"num_seeds must be an integer >= 1, got {num_seeds}")
+    lo = np.array(model.lowerPositionLimit, dtype=np.float64)
+    hi = np.array(model.upperPositionLimit, dtype=np.float64)
+    bounded = np.isfinite(lo) & np.isfinite(hi) & (hi > lo)
+    circle = np.zeros(model.nq, dtype=bool)
+    for j in model.joints:
+        if j.kind == "revolute" and not np.isfinite(lo[j.idx_q]) and not np.isfinite(hi[j.idx_q]):
+            circle[j.idx_q] = True
+    lo = np.where(circle, -math.pi, np.where(bounded, lo, 0.0))
+    hi = np.where(circle, math.pi, np.where(bounded, hi, 0.0))
+    B, S = q.shape[0], int(num_seeds)
+    u = torch.rand((B, S - 1, model.nq), generator=generator, dtype=torch.float64, device=q.device)
+    lo_t = torch.as_tensor(lo, device=q.device)
+    hi_t = torch.as_tensor(hi, device=q.device)
+    x = (lo_t + (hi_t - lo_t) * u).to(q.dtype)
+    # strictly inside after the rounding to q's dtype
+    inside_lo = torch.nextafter(lo_t.to(q.dtype), hi_t.to(q.dtype))
+    inside_hi = torch.nextafter(hi_t.to(q.dtype), lo_t.to(q.dtype))
+    x = torch.minimum(torch.maximum(x, inside_lo), inside_hi)
+    draw = torch.as_tensor(bounded | circle, device=q.device)
+    rest = torch.where(draw, x, q[:, None, :].expand(B, S - 1, model.nq))
+    return torch.cat([q[:, None, :], rest], dim=1).contiguous()

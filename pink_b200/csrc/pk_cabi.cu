@@ -17,6 +17,7 @@
 #include "pk_chain.cuh"
 #include "pk_coop_kernel.cuh"
 #include "pk_generic.cuh"
+#include "pk_multistart.cuh"
 #include "pk_select.hpp"
 
 namespace {
@@ -864,7 +865,7 @@ struct SmemGrant {
   std::mutex mu;
   size_t bytes[64] = {};
 };
-SmemGrant g_tree_smem, g_tree_rollout_smem, g_tree_converge_smem;
+SmemGrant g_tree_smem, g_tree_rollout_smem, g_tree_converge_smem, g_tree_multistart_smem;
 
 // A tree kernel: one instance per warp, `plan.words` floats of dynamic shared memory per warp.
 template <class... Params, class... Args>
@@ -1258,6 +1259,65 @@ extern "C" int pk_converge_prepared(const PkModel* m, const PkProblem* pr, const
   pk::with_generic(sel.generic_class, [&](auto nj, auto nv) {
     pk::ik_generic_converge_kernel<decltype(nj)::value, decltype(nv)::value><<<(unsigned)grid, block, 0, stream>>>(
         m->dev, pr->P, q, targets, task_mask, tol, max_steps, q_out, err, steps, status, B);
+  });
+  return launched();
+}
+
+extern "C" int pk_converge_multistart_prepared(const PkModel* m, const PkProblem* pr, const float* q_seeds,
+                                               int32_t num_seeds, const float* targets, uint32_t task_mask, float tol,
+                                               int32_t max_steps, float* q_out, float* err, int32_t* seed,
+                                               int32_t* steps, int32_t* status, int64_t B, void* stream_) {
+  if (check_common(m, q_seeds, B)) return 1;
+  if (!pr) return fail("null problem");
+  const std::string aerr = pk::check_converge_args(pr->P, task_mask, tol, max_steps);
+  if (!aerr.empty()) return fail(aerr);
+  const pk::Selection& sel = pr->sel;
+  const std::string serr = pk::check_multistart_seeds(sel, num_seeds);
+  if (!serr.empty()) return fail(serr);
+  const int S = num_seeds;
+  if (B > (int64_t)2147483647 * 32 / S) return fail("batch too large");
+  if (B > 0 && !q_out) return fail("null q_out");
+  if (B > 0 && pr->P.target_stride > 0 && !targets) return fail("null targets");
+  if (B == 0) return 0;
+  cudaStream_t stream = (cudaStream_t)stream_;
+  if (sel.path == pk::kPathTree) {
+    if (B > 2147483647) return fail("batch too large");
+    const pk::MultistartTreeLayout T = pk::multistart_tree_layout(sel.plan);
+    const size_t smem = T.smem_bytes(S);
+    {
+      std::lock_guard<std::mutex> lock(g_tree_multistart_smem.mu);
+      const int dev = (m->device >= 0 && m->device < 64) ? m->device : 0;
+      if (smem > g_tree_multistart_smem.bytes[dev] || m->device >= 64) {
+        PK_CUDA(cudaFuncSetAttribute(pk::ik_tree_multistart_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                     (int)smem));
+        g_tree_multistart_smem.bytes[dev] = smem;
+      }
+    }
+    pk::ik_tree_multistart_kernel<<<(unsigned)B, 32 * S, smem, stream>>>(m->dev, pr->P, T.plan, T.o_v, T.o_q, q_seeds,
+                                                                         S, targets, task_mask, tol, max_steps, q_out,
+                                                                         err, seed, steps, status, B);
+    return launched();
+  }
+  const int64_t rows = B * S;
+  if (sel.path == pk::kPathChain) {
+    const unsigned emask = pk::chain_task_mask(pr->P, task_mask, sel.nft);
+    const int block = 128;
+    const int64_t grid = (rows + block - 1) / block;
+    pk::with_nj(sel.nj, [&](auto nj) {
+      constexpr int NJ = decltype(nj)::value;
+      pk::with_nft(sel.nft, [&](auto nft) {
+        pk::ik_chain_multistart_kernel<NJ, decltype(nft)::value><<<(unsigned)grid, block, 0, stream>>>(
+            *reinterpret_cast<const pk::ChainParams<NJ>*>(pr->chain_params), q_seeds, S, targets, emask, tol,
+            max_steps, q_out, err, seed, steps, status, B);
+      });
+    });
+    return launched();
+  }
+  const int block = 64;
+  const int64_t grid = (rows + block - 1) / block;
+  pk::with_generic(sel.generic_class, [&](auto nj, auto nv) {
+    pk::ik_generic_multistart_kernel<decltype(nj)::value, decltype(nv)::value><<<(unsigned)grid, block, 0, stream>>>(
+        m->dev, pr->P, q_seeds, S, targets, task_mask, tol, max_steps, q_out, err, seed, steps, status, B);
   });
   return launched();
 }

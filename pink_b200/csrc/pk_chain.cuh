@@ -282,6 +282,30 @@ PK_HD void ik_step_chain(const ChainParams<NJ>& P, const float (&q)[NJ], const f
   status_out = status;
 }
 
+// The rest of a converge step after C.assemble<true> returned `status` and `skip`: the QP of
+// ik_step_chain, its status ORed into st_all.  Returns false, with q unchanged, when the freeze
+// rule of the rollouts fires; otherwise moves q to q (+) v dt.
+template <int NJ, int NFT>
+PK_HD bool converge_chain_advance(const ChainParams<NJ>& P, ChainStep<NJ, NFT>& C, int status, bool skip,
+                                  float (&q)[NJ], int& st_all, int flags) {
+  int st = status;
+  float x[NJ];
+#pragma unroll
+  for (int j = 0; j < NJ; ++j) x[j] = 0.f;
+  if (!skip && !(st & PK_STATUS_NO_SOLUTION))
+    st |= BoxLSQChol<6 * NFT, NJ>::run(C.A, C.b, C.d, C.beta, C.lo, C.hi, x, flags);
+  float sum = 0.f;
+#pragma unroll
+  for (int j = 0; j < NJ; ++j) sum += x[j];
+  const bool finite = fabsf(sum) < 3.0e38f;
+  if (!finite) st |= PK_STATUS_NO_SOLUTION;
+  st_all |= st & 0xff;
+  if (step_failed(st_all, P.safety_break)) return false;
+#pragma unroll
+  for (int k = 0; k < NJ; ++k) q[k] = fmaf(finite ? x[k] * P.inv_dt : 0.f, P.dt, q[k]);  // q (+) v dt = q + v dt
+  return true;
+}
+
 // Solve to a tolerance (pk_converge_prepared), one instance, q in registers.  For s = 0, 1, ...:
 // err(q_s) = the largest |e_t|_2 of the tasks of `emask` (chain slots, see assemble); stop at
 // q_s when err <= tol or s == max_steps; otherwise take the step ik_step_chain takes (its status
@@ -300,25 +324,10 @@ PK_HD void converge_chain(const ChainParams<NJ>& P, float (&q)[NJ], const float*
     const int status = C.template assemble<true>(P, q, trow, skip, emask, &e);
     err = e;
     if (e <= tol || s == max_steps) break;
-    // the rest of ik_step_chain
-    int st = status;
-    float x[NJ];
-#pragma unroll
-    for (int j = 0; j < NJ; ++j) x[j] = 0.f;
-    if (!skip && !(st & PK_STATUS_NO_SOLUTION))
-      st |= BoxLSQChol<6 * NFT, NJ>::run(C.A, C.b, C.d, C.beta, C.lo, C.hi, x, flags);
-    float sum = 0.f;
-#pragma unroll
-    for (int j = 0; j < NJ; ++j) sum += x[j];
-    const bool finite = fabsf(sum) < 3.0e38f;
-    if (!finite) st |= PK_STATUS_NO_SOLUTION;
-    st_all |= st & 0xff;
-    if (step_failed(st_all, P.safety_break)) {
+    if (!converge_chain_advance(P, C, status, skip, q, st_all, flags)) {
       ++s;
       break;
     }
-#pragma unroll
-    for (int k = 0; k < NJ; ++k) q[k] = fmaf(finite ? x[k] * P.inv_dt : 0.f, P.dt, q[k]);  // q (+) v dt = q + v dt
   }
   steps = s;
   status_out = st_all;

@@ -446,10 +446,11 @@ struct Generic {
 
   // One step. `q` [nq], `trow` per-instance targets.
   // ERR (converge_generic): also the stop test `ct` on the task errors, made before the QP; a
-  // step that stops there writes only *out.status (and ct).
-  template <bool ERR = false>
+  // step that stops there writes only *out.status (and ct).  Test: the stop rule, ct->decide(err)
+  // (ConvergeTest: this instance's own; the multi-start kernel's decides for a group of seeds).
+  template <bool ERR = false, class Test = ConvergeTest>
   PK_HD void step(const DevModel& M, const DevProblem& P, const float* q, const float* trow, const GenericOut& out,
-                  ConvergeTest* ct = nullptr) {
+                  Test* ct = nullptr) {
     const int nv = M.nv;
     const int rq = M.free_flyer ? 7 : 0;
     const int rv = M.free_flyer ? 6 : 0;
@@ -554,8 +555,7 @@ struct Generic {
     }
     if (K > kGenericMaxRows) { status |= PK_STATUS_NOT_POSDEF; K = kGenericMaxRows; }
     if constexpr (ERR) {
-      ct->err = emax;
-      ct->stop = emax <= ct->tol || ct->last;
+      ct->decide(emax);
       ct->status = status;
       if (ct->stop) {
         if (out.status) *out.status = status;

@@ -191,6 +191,11 @@ inline std::string check_converge_args(const DevProblem& P, uint32_t mask, float
   return "";
 }
 
+// Seeds per target of pk_converge_multistart_prepared: a power of two that fits one warp, so that
+// a group of seeds is S adjacent lanes.
+constexpr int kMaxSeeds = 32;
+inline bool valid_num_seeds(int S) { return S >= 1 && S <= kMaxSeeds && (S & (S - 1)) == 0; }
+
 // Problem of the forward-kinematics and frame-Jacobian exports: no tasks, no limits.
 inline DevProblem kinematics_problem() {
   DevProblem P;

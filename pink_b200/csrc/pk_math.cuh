@@ -386,6 +386,8 @@ PK_HD float err_max(float m, float n) { return (n > m || n != n) ? n : m; }
 // take it: in mask (bit t: task t of the problem), tol, last (s == max_steps); out the error,
 // max over the tasks of mask of |e_t|_2 (unweighted, gain-free), whether the loop stops here
 // (the step then returns before its QP), and the step's status (the same on every lane).
+// The bodies take the test type as a template parameter: decide() is the stop rule, called
+// where the error is known (the multi-start kernels pass a test that decides for a group).
 struct ConvergeTest {
   unsigned mask;
   float tol;
@@ -393,6 +395,19 @@ struct ConvergeTest {
   float err;
   bool stop;
   int status;
+  PK_HD void decide(float e) {
+    err = e;
+    stop = e <= tol || last;
+  }
 };
+
+// Order of the seeds of a multi-start group (pk_converge_multistart_prepared): seed a (error ea)
+// comes before seed b when its error is smaller, a NaN error counting as +inf, ties going to the
+// lower seed index.  The winner is the first seed in this order.
+PK_HD bool seed_before(float ea, int a, float eb, int b) {
+  ea = ea != ea ? INFINITY : ea;
+  eb = eb != eb ? INFINITY : eb;
+  return ea < eb || (ea == eb && a < b);
+}
 
 }  // namespace pk

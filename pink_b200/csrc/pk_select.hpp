@@ -73,6 +73,41 @@ inline unsigned chain_task_mask(const DevProblem& P, unsigned mask, int nft) {
   return out;
 }
 
+// Multi-start on joint trees (pk_converge_multistart_prepared): one target per CTA, one seed per
+// warp.  A warp's workspace is the plan's words, then the step's v, then the seed's q (each
+// 4-word aligned); after the S workspaces come the group's slots, two rounds of S errors and S
+// failed flags.  The CTA's dynamic shared memory is capped at kCtaSmemBytes, the opt-in limit of
+// sm_90.
+constexpr int kTreeMaxSeeds = 8;
+constexpr size_t kCtaSmemBytes = 227 * 1024;
+struct MultistartTreeLayout {
+  TreePlan plan;  // plan.words: the whole per-warp workspace
+  int o_v, o_q;
+  size_t smem_bytes(int S) const { return ((size_t)plan.words * S + 4 * (size_t)S) * 4; }
+};
+inline MultistartTreeLayout multistart_tree_layout(const TreePlan& plan) {
+  MultistartTreeLayout T;
+  T.plan = plan;
+  T.o_v = T.plan.words;
+  T.plan.words += (plan.nv + 3) & ~3;
+  T.o_q = T.plan.words;
+  T.plan.words += (plan.nq + 3) & ~3;
+  return T;
+}
+
+// Arguments of pk_converge_multistart_prepared beyond check_converge_args; "" when valid.
+inline std::string check_multistart_seeds(const Selection& sel, int S) {
+  if (!valid_num_seeds(S)) return "num_seeds must be 1, 2, 4, 8, 16 or 32";
+  if (sel.path == kPathTree) {
+    if (S > kTreeMaxSeeds) return "num_seeds must be at most 8 on the tree kernel (one warp per seed in one CTA)";
+    const size_t bytes = multistart_tree_layout(sel.plan).smem_bytes(S);
+    if (bytes > kCtaSmemBytes)
+      return "num_seeds = " + std::to_string(S) + " needs " + std::to_string(bytes) +
+             " B of shared memory on the tree kernel, more than one CTA's " + std::to_string(kCtaSmemBytes) + " B";
+  }
+  return "";
+}
+
 // f(std::integral_constant<int, N>) for the run-time value: the chain kernels' joint count
 // (2..7, chain_eligible), frame-task count (0..2), sub-warp lanes (a coop_has_variant), the
 // general path's <NJMAX, NVMAX>.

@@ -629,11 +629,13 @@ struct TreeStep {
   // ---- the whole step ----------------------------------------------------------------
   // ERR (converge): also the stop test `ct` on the task errors, reduced across the warp and made
   // before the rows of A; a step that stops there, or whose instance is outside its limits with
-  // safety_break, returns with v = 0.  ct->status is the step's status on every lane.
-  template <bool ERR = false>
+  // safety_break, returns with v = 0.  ct->status is the step's status on every lane.  Test: the
+  // stop rule, ct->decide(err), called by the whole warp (ConvergeTest: this instance's own; the
+  // multi-start kernel's decides for the CTA's group of seeds, with a barrier).
+  template <bool ERR = false, class Test = ConvergeTest>
   static PK_HD void run(const DevModel& M, const DevProblem& P, const TreePlan& L, const float* __restrict__ qg,
                         const float* __restrict__ tg, float* W, float* __restrict__ vg, int32_t* status_out,
-                        ConvergeTest* ct = nullptr) {
+                        Test* ct = nullptr) {
     const int nj = L.nj, nv = L.nv, rq = L.rq, rv = L.rv;
     float* qs = W + L.o_q;
     float* ts = W + L.o_t;
@@ -816,8 +818,7 @@ struct TreeStep {
         }
         emax = err_max(emax, sqrtf(n2));
       }
-      ct->err = emax;
-      ct->stop = emax <= ct->tol || ct->last;
+      ct->decide(emax);
       ct->status = status;
       if (ct->stop || (status && P.safety_break)) {
         PK_LANES(l) {
