@@ -358,22 +358,6 @@ __device__ __forceinline__ bool chain_copy_row(float* dst, const float* src, int
   return diff == 0u;
 }
 
-// Records of step s of a trajectory (thread-per-instance chain kernel); `frozen`: v row of zeros.
-template <int NJ>
-__device__ __forceinline__ void chain_record(const Trajectory& T, int s, int64_t B, int64_t i, const float (&qi)[NJ],
-                                             const float (&vi)[NJ], int st_all, bool frozen) {
-  const int64_t r = (int64_t)s * B + i;
-  if (T.q) {
-#pragma unroll
-    for (int k = 0; k < NJ; ++k) T.q[r * NJ + k] = qi[k];
-  }
-  if (T.v) {
-#pragma unroll
-    for (int k = 0; k < NJ; ++k) T.v[r * NJ + k] = frozen ? 0.f : vi[k];
-  }
-  if (T.status) T.status[r] = st_all;
-}
-
 // T: per-step targets and records of a trajectory call, read by the plain instantiation only.
 // The PDL protocol validates one copied targets row after the wait and stores nothing before
 // it, so it cannot cover K rows or per-step stores: trajectory calls with a step stride or
@@ -418,32 +402,7 @@ __global__ void __launch_bounds__(128, 4)
   int st_all;
 #pragma unroll 1
   for (int pass = 0;; ++pass) {
-    st_all = 0;
-#pragma unroll
-    for (int k = 0; k < NJ; ++k) vi[k] = 0.f;
-#pragma unroll 1
-    for (int step_no = 0; step_no < n_steps; ++step_no) {
-      const bool frozen =
-          (st_all & (PK_STATUS_NO_SOLUTION | PK_STATUS_NOT_POSDEF)) || ((st_all & PK_STATUS_OUT_OF_LIMITS) && P.safety_break);
-      if (frozen) {
-        if constexpr (!PDL) {
-#pragma unroll 1
-          for (int s = step_no; s < n_steps; ++s) chain_record<NJ>(T, s, B, i, qi, vi, st_all, true);
-        }
-        break;
-      }
-      int st;
-      ik_step_chain<NJ, NFT>(P, qi, trow, vi, st, flags);
-      st_all |= st & 0xff;
-      if (n_steps > 1 || q_out) {
-#pragma unroll
-        for (int k = 0; k < NJ; ++k) qi[k] = fmaf(vi[k], P.dt, qi[k]);  // 1-dof joints: q (+) v dt = q + v dt
-      }
-      if constexpr (!PDL) {
-        trow += T.target_step;
-        chain_record<NJ>(T, step_no, B, i, qi, vi, st_all, false);
-      }
-    }
+    st_all = rollout_chain<NJ, NFT, !PDL>(P, qi, trow, vi, n_steps, q_out != nullptr, flags, T, B, i);
     if constexpr (!PDL) {
       break;
     } else {
@@ -553,22 +512,8 @@ __global__ void __launch_bounds__(64) ik_generic_kernel(const DevModel M, const 
   G.step(M, P, A.q + i * M.nq, A.targets ? A.targets + i * (int64_t)P.target_stride : nullptr, out);
 }
 
-// Records of step s of a trajectory from an instance's q / v rows (`n` threads from `lane`).
-__device__ __forceinline__ void record_rows(const Trajectory& T, int s, int64_t B, int64_t i, int nq, int nv,
-                                            const float* qrow, const float* vrow, int st_all, bool frozen,
-                                            int lane, int n) {
-  const int64_t r = (int64_t)s * B + i;
-  if (T.q)
-    for (int k = lane; k < nq; k += n) T.q[r * nq + k] = qrow[k];
-  if (T.v)
-    for (int k = lane; k < nv; k += n) T.v[r * nv + k] = frozen ? 0.f : vrow[k];
-  if (T.status && lane == 0) T.status[r] = st_all;
-}
-
-// Trajectory rollout of the general path in one launch: per thread, n_steps iterations of
-// Generic::step and q (+) v dt on the instance's q_out row in place, with the freeze rule of the
-// chain kernel (an instance that fails a step is frozen after it; status = OR over the steps
-// that ran).
+// Trajectory rollout of the general path in one launch: rollout_generic per thread on the
+// instance's q_out row in place.
 template <int NJMAX, int NVMAX>
 __global__ void __launch_bounds__(64)
     ik_generic_rollout_kernel(const DevModel M, const __grid_constant__ DevProblem P, const float* q,
@@ -576,29 +521,11 @@ __global__ void __launch_bounds__(64)
                               int32_t* __restrict__ status, int64_t B, const __grid_constant__ Trajectory T) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= B) return;
-  const int nq = M.nq, nv = M.nv;
+  const int nq = M.nq;
   float* qrow = q_out + i * nq;
-  float* vrow = v + i * nv;
   for (int k = 0; k < nq; ++k) qrow[k] = q[i * nq + k];
-  int32_t st = 0;
-  GenericOut out{};
-  out.v = vrow;
-  out.status = &st;
-  out.task_index = -1;
   Generic<NJMAX, NVMAX> G;
-  int st_all = 0;
-  for (int s = 0; s < n_steps; ++s) {
-    const bool frozen =
-        (st_all & (PK_STATUS_NO_SOLUTION | PK_STATUS_NOT_POSDEF)) || ((st_all & PK_STATUS_OUT_OF_LIMITS) && P.safety_break);
-    if (frozen) {
-      record_rows(T, s, B, i, nq, nv, qrow, vrow, st_all, true, 0, 1);
-      continue;
-    }
-    G.step(M, P, qrow, targets ? targets + s * T.target_step + i * (int64_t)P.target_stride : nullptr, out);
-    st_all |= st;
-    integrate_configuration(nq, M.free_flyer, qrow, vrow, P.dt, qrow);
-    record_rows(T, s, B, i, nq, nv, qrow, vrow, st_all, false, 0, 1);
-  }
+  const int st_all = rollout_generic(G, M, P, qrow, v + i * M.nv, targets, n_steps, T, B, i);
   if (status) status[i] = st_all;
 }
 
@@ -647,14 +574,9 @@ __global__ void __launch_bounds__(32 * kTreeWarpsPerBlock, PK_TREE_MIN_BLOCKS)
                 status ? status + i : nullptr);
 }
 
-// Closed-loop rollout of the tree kernel in ONE launch: n_steps iterations of
-// v = solve_ik(q); q <- q (+) v dt (pink/configuration.py:285-293 after pink/solve_ik.py:274)
-// per warp, the instance's q / v rows re-read by the warp that wrote them (they stay in
-// L1 / L2; the per-step launch pair and its two full passes over HBM are gone).  An instance
-// that fails a step (no solution / outside limits with safety_break) is frozen, as on chains.
-// T: per-step targets rows and records of a trajectory call (pk_rollout_trajectory_prepared); the
-// lanes store the q / v rows into the records after every step, and a frozen instance's warp
-// fills its remaining steps (q unchanged, v = 0, the same status).
+// Closed-loop rollout of the tree kernel in ONE launch: TreeStep::rollout per warp on the
+// instance's q_out row in place, the q / v rows re-read by the warp that wrote them (they stay in
+// L1 / L2; the per-step launch pair and its two full passes over HBM are gone).
 __global__ void __launch_bounds__(32 * kTreeWarpsPerBlock)
     ik_tree_rollout_kernel(const DevModel M, const __grid_constant__ DevProblem P, const __grid_constant__ TreePlan L,
                            const float* __restrict__ q, const float* __restrict__ targets, int n_steps,
@@ -666,24 +588,9 @@ __global__ void __launch_bounds__(32 * kTreeWarpsPerBlock)
   if (i >= B) return;
   float* W = tree_smem + (size_t)warp * L.words;
   float* qrow = q_out + i * L.nq;
-  float* vrow = v + i * L.nv;
   for (int k = lane; k < L.nq; k += 32) qrow[k] = q[i * L.nq + k];
   __syncwarp();
-  int st_all = 0;
-  int s = 0;
-  while (s < n_steps) {
-    int32_t st = 0;
-    TreeStep::run(M, P, L, qrow, targets ? targets + s * T.target_step + i * (int64_t)L.stride : nullptr, W, vrow, &st);
-    __syncwarp();
-    st = __shfl_sync(0xffffffffu, st, 0);  // run() reports through lane 0
-    st_all |= st;
-    const bool failed = (st & (PK_STATUS_NO_SOLUTION | PK_STATUS_NOT_POSDEF)) || ((st & PK_STATUS_OUT_OF_LIMITS) && P.safety_break);
-    if (!failed && lane == 0) integrate_configuration(L.nq, M.free_flyer, qrow, vrow, P.dt, qrow);
-    __syncwarp();
-    record_rows(T, s++, B, i, L.nq, L.nv, qrow, vrow, st_all, false, lane, 32);
-    if (failed) break;
-  }
-  for (; s < n_steps; ++s) record_rows(T, s, B, i, L.nq, L.nv, qrow, vrow, st_all, true, lane, 32);
+  const int st_all = TreeStep::rollout(M, P, L, qrow, targets, W, v + i * L.nv, n_steps, T, B, i);
   if (status && lane == 0) status[i] = st_all;
 }
 
@@ -867,11 +774,10 @@ struct SmemGrant {
 };
 SmemGrant g_tree_smem, g_tree_rollout_smem, g_tree_converge_smem, g_tree_multistart_smem;
 
-// A tree kernel: one instance per warp, `plan.words` floats of dynamic shared memory per warp.
+// A tree kernel with `smem` bytes of dynamic shared memory per CTA, opted into beyond the default.
 template <class... Params, class... Args>
-int launch_tree(void (*kernel)(Params...), SmemGrant& grant, const PkModel* m, const pk::TreePlan& plan, int64_t B,
+int launch_tree(void (*kernel)(Params...), SmemGrant& grant, const PkModel* m, int64_t grid, int block, size_t smem,
                 cudaStream_t stream, const Args&... args) {
-  const size_t smem = (size_t)plan.words * 4 * pk::kTreeWarpsPerBlock;
   {
     std::lock_guard<std::mutex> lock(grant.mu);
     const int dev = (m->device >= 0 && m->device < 64) ? m->device : 0;
@@ -880,9 +786,16 @@ int launch_tree(void (*kernel)(Params...), SmemGrant& grant, const PkModel* m, c
       grant.bytes[dev] = smem;
     }
   }
-  const int64_t grid = (B + pk::kTreeWarpsPerBlock - 1) / pk::kTreeWarpsPerBlock;
-  kernel<<<(unsigned)grid, 32 * pk::kTreeWarpsPerBlock, smem, stream>>>(args...);
+  kernel<<<(unsigned)grid, block, smem, stream>>>(args...);
   return launched();
+}
+
+// A tree kernel with one instance per warp and `plan.words` floats of dynamic shared memory per warp.
+template <class... Params, class... Args>
+int launch_tree_warps(void (*kernel)(Params...), SmemGrant& grant, const PkModel* m, const pk::TreePlan& plan,
+                      int64_t B, cudaStream_t stream, const Args&... args) {
+  return launch_tree(kernel, grant, m, (B + pk::kTreeWarpsPerBlock - 1) / pk::kTreeWarpsPerBlock,
+                     32 * pk::kTreeWarpsPerBlock, (size_t)plan.words * 4 * pk::kTreeWarpsPerBlock, stream, args...);
 }
 
 }  // namespace
@@ -1005,8 +918,8 @@ int solve_device(const PkModel* m, const PkProblem& pr, const float* q, const fl
   if (B == 0) return 0;
   if (pr.sel.path == pk::kPathChain) return launch_chain_prepared(pr, q, targets, v, status, B, stream, 1, nullptr, nullptr);
   if (pr.sel.path == pk::kPathTree)
-    return launch_tree(pk::ik_tree_kernel, g_tree_smem, m, pr.sel.plan, B, stream, m->dev, pr.P, pr.sel.plan, q,
-                       targets, v, status, B);
+    return launch_tree_warps(pk::ik_tree_kernel, g_tree_smem, m, pr.sel.plan, B, stream, m->dev, pr.P, pr.sel.plan,
+                             q, targets, v, status, B);
   pk::GenericArgs A{};
   A.q = q;
   A.targets = targets;
@@ -1186,8 +1099,8 @@ extern "C" int pk_rollout_prepared(const PkModel* m, const PkProblem* pr, const 
   if (pr->sel.path == pk::kPathChain)
     return launch_chain_prepared(*pr, q, targets, v, status, B, stream, n_steps, q_out, nullptr);
   if (pr->sel.path == pk::kPathTree)  // joint trees: the whole loop in one launch of the warp kernel
-    return launch_tree(pk::ik_tree_rollout_kernel, g_tree_rollout_smem, m, pr->sel.plan, B, stream, m->dev, pr->P,
-                       pr->sel.plan, q, targets, n_steps, q_out, v, status, B, kNoTrajectory);
+    return launch_tree_warps(pk::ik_tree_rollout_kernel, g_tree_rollout_smem, m, pr->sel.plan, B, stream, m->dev,
+                             pr->P, pr->sel.plan, q, targets, n_steps, q_out, v, status, B, kNoTrajectory);
   // other models: the same closed loop as separate launches (solve, then integrate in place)
   if (q_out != q) PK_CUDA(cudaMemcpyAsync(q_out, q, sizeof(float) * B * m->nq, cudaMemcpyDeviceToDevice, stream));
   for (int s = 0; s < n_steps; ++s) {
@@ -1213,8 +1126,8 @@ extern "C" int pk_rollout_trajectory_prepared(const PkModel* m, const PkProblem*
   if (pr->sel.path == pk::kPathChain)
     return launch_chain_prepared(*pr, q, targets, v, status, B, stream, n_steps, q_out, nullptr, traj);
   if (pr->sel.path == pk::kPathTree)
-    return launch_tree(pk::ik_tree_rollout_kernel, g_tree_rollout_smem, m, pr->sel.plan, B, stream, m->dev, pr->P,
-                       pr->sel.plan, q, targets, n_steps, q_out, v, status, B, traj);
+    return launch_tree_warps(pk::ik_tree_rollout_kernel, g_tree_rollout_smem, m, pr->sel.plan, B, stream, m->dev,
+                             pr->P, pr->sel.plan, q, targets, n_steps, q_out, v, status, B, traj);
   return launch_generic_rollout(m, pr->sel.generic_class, pr->P, q, targets, n_steps, q_out, v, status, B, stream,
                                 traj);
 }
@@ -1251,8 +1164,8 @@ extern "C" int pk_converge_prepared(const PkModel* m, const PkProblem* pr, const
     pk::TreePlan plan = sel.plan;
     const int o_v = plan.words;
     plan.words += (plan.nv + 3) & ~3;
-    return launch_tree(pk::ik_tree_converge_kernel, g_tree_converge_smem, m, plan, B, stream, m->dev, pr->P, plan, o_v,
-                       q, targets, task_mask, tol, (int)max_steps, q_out, err, steps, status, B);
+    return launch_tree_warps(pk::ik_tree_converge_kernel, g_tree_converge_smem, m, plan, B, stream, m->dev, pr->P, plan,
+                             o_v, q, targets, task_mask, tol, (int)max_steps, q_out, err, steps, status, B);
   }
   const int block = 64;
   const int64_t grid = (B + block - 1) / block;
@@ -1283,20 +1196,9 @@ extern "C" int pk_converge_multistart_prepared(const PkModel* m, const PkProblem
   if (sel.path == pk::kPathTree) {
     if (B > 2147483647) return fail("batch too large");
     const pk::MultistartTreeLayout T = pk::multistart_tree_layout(sel.plan);
-    const size_t smem = T.smem_bytes(S);
-    {
-      std::lock_guard<std::mutex> lock(g_tree_multistart_smem.mu);
-      const int dev = (m->device >= 0 && m->device < 64) ? m->device : 0;
-      if (smem > g_tree_multistart_smem.bytes[dev] || m->device >= 64) {
-        PK_CUDA(cudaFuncSetAttribute(pk::ik_tree_multistart_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                     (int)smem));
-        g_tree_multistart_smem.bytes[dev] = smem;
-      }
-    }
-    pk::ik_tree_multistart_kernel<<<(unsigned)B, 32 * S, smem, stream>>>(m->dev, pr->P, T.plan, T.o_v, T.o_q, q_seeds,
-                                                                         S, targets, task_mask, tol, max_steps, q_out,
-                                                                         err, seed, steps, status, B);
-    return launched();
+    return launch_tree(pk::ik_tree_multistart_kernel, g_tree_multistart_smem, m, B, 32 * S, T.smem_bytes(S), stream,
+                       m->dev, pr->P, T.plan, T.o_v, T.o_q, q_seeds, S, targets, task_mask, tol, (int)max_steps,
+                       q_out, err, seed, steps, status, B);
   }
   const int64_t rows = B * S;
   if (sel.path == pk::kPathChain) {

@@ -333,4 +333,56 @@ PK_HD void converge_chain(const ChainParams<NJ>& P, float (&q)[NJ], const float*
   status_out = st_all;
 }
 
+// Records of step s of a trajectory (thread-per-instance chain kernel); `frozen`: v row of zeros.
+template <int NJ>
+PK_HD void chain_record(const Trajectory& T, int s, int64_t B, int64_t i, const float (&qi)[NJ],
+                        const float (&vi)[NJ], int st_all, bool frozen) {
+  const int64_t r = (int64_t)s * B + i;
+  if (T.q) {
+#pragma unroll
+    for (int k = 0; k < NJ; ++k) T.q[r * NJ + k] = qi[k];
+  }
+  if (T.v) {
+#pragma unroll
+    for (int k = 0; k < NJ; ++k) T.v[r * NJ + k] = frozen ? 0.f : vi[k];
+  }
+  if (T.status) T.status[r] = st_all;
+}
+
+// Closed-loop rollout of instance i (ik_chain_kernel): n_steps iterations of ik_step_chain, each
+// followed by q <- q (+) v dt when n_steps > 1 or `integrate`; an instance whose statuses so far
+// fail the freeze rule takes no further step.  Returns the OR of the statuses of the steps that
+// ran; v is the last step's.  RECORD: the targets row advances by T.target_step after every step,
+// and the records of T are stored (a frozen instance fills its remaining steps with q unchanged
+// and v = 0).
+template <int NJ, int NFT, bool RECORD>
+PK_HD int rollout_chain(const ChainParams<NJ>& P, float (&qi)[NJ], const float* trow, float (&vi)[NJ], int n_steps,
+                        bool integrate, int flags, const Trajectory& T, int64_t B, int64_t i) {
+  int st_all = 0;
+#pragma unroll
+  for (int k = 0; k < NJ; ++k) vi[k] = 0.f;
+#pragma unroll 1
+  for (int step_no = 0; step_no < n_steps; ++step_no) {
+    if (step_failed(st_all, P.safety_break)) {
+      if constexpr (RECORD) {
+#pragma unroll 1
+        for (int s = step_no; s < n_steps; ++s) chain_record<NJ>(T, s, B, i, qi, vi, st_all, true);
+      }
+      break;
+    }
+    int st;
+    ik_step_chain<NJ, NFT>(P, qi, trow, vi, st, flags);
+    st_all |= st & 0xff;
+    if (n_steps > 1 || integrate) {
+#pragma unroll
+      for (int k = 0; k < NJ; ++k) qi[k] = fmaf(vi[k], P.dt, qi[k]);  // 1-dof joints: q (+) v dt = q + v dt
+    }
+    if constexpr (RECORD) {
+      trow += T.target_step;
+      chain_record<NJ>(T, step_no, B, i, qi, vi, st_all, false);
+    }
+  }
+  return st_all;
+}
+
 }  // namespace pk

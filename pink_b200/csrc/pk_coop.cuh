@@ -686,4 +686,54 @@ PK_HD void ik_step_coop(const Group<L>& G, const CoopParams<CoopStep<NJ, NFT, L>
   status_out = status;
 }
 
+// Closed-loop rollout of instance `inst` (ik_coop_kernel), the loop of rollout_chain (pk_chain.cuh)
+// with ik_step_coop: S[h].q in, where the instance ended out; S[h].x the last step's velocity.
+// Each lane stores the joints it owns into the records of T, lane 0 of the group the status.
+template <int NJ, int NFT, int L, class JC>
+PK_HD int rollout_coop(const Group<L>& G, const CoopParams<CoopStep<NJ, NFT, L>::NJP>& P, JC jc, const float* trow,
+                       GVar<typename CoopStep<NJ, NFT, L>::Lane, L>& S, int n_steps, bool integrate,
+                       const Trajectory& T, int64_t B, int64_t inst) {
+  constexpr int NC = CoopStep<NJ, NFT, L>::NC;
+  // records of step s: the lane's joints of q and v, the status from lane 0 of the group
+  auto record = [&](int s, int st_all, bool frozen) {
+    const int64_t r = (int64_t)s * B + inst;
+    PK_GLANES(G, h) {
+#pragma unroll
+      for (int k = 0; k < NC; ++k) {
+        const int j = h * NC + k;
+        if (j < NJ) {
+          if (T.q) T.q[r * NJ + j] = S[h].q[k];
+          if (T.v) T.v[r * NJ + j] = frozen ? 0.f : S[h].x[k];
+        }
+      }
+      if (T.status && h == 0) T.status[r] = st_all;
+    }
+  };
+  int st_all = 0;
+  PK_GLANES(G, h) {
+#pragma unroll
+    for (int k = 0; k < NC; ++k) S[h].x[k] = 0.f;
+  }
+#pragma unroll 1
+  for (int step_no = 0; step_no < n_steps; ++step_no) {
+    if (step_failed(st_all, P.safety_break)) {
+#pragma unroll 1
+      for (int s = step_no; s < n_steps; ++s) record(s, st_all, true);
+      break;
+    }
+    int st;
+    ik_step_coop<NJ, NFT, L>(G, P, jc, trow, S, st);
+    st_all |= st & 0xff;
+    if (n_steps > 1 || integrate) {
+      PK_GLANES(G, h) {
+#pragma unroll
+        for (int k = 0; k < NC; ++k) S[h].q[k] = fmaf(S[h].x[k], P.dt, S[h].q[k]);  // 1-dof joints: q + v dt
+      }
+    }
+    trow += T.target_step;
+    record(step_no, st_all, false);
+  }
+  return st_all;
+}
+
 }  // namespace pk

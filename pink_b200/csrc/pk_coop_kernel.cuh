@@ -1,9 +1,8 @@
 // Device wrapper of pk_coop.cuh: L lanes per instance, 128 threads per CTA.
-// n_steps > 1: closed-loop rollout, q <- q (+) v dt after every step with q kept in
-// registers (pink/configuration.py:285-293 after pink/solve_ik.py:274); an instance that
+// n_steps > 1: closed-loop rollout (rollout_coop), q <- q (+) v dt after every step with q kept
+// in registers (pink/configuration.py:285-293 after pink/solve_ik.py:274); an instance that
 // fails a step (no solution / outside limits with safety_break) is frozen.  T: per-step targets
-// rows and records of a trajectory call (pk_rollout_trajectory_prepared); each lane stores the
-// joints it owns, and a frozen instance fills its remaining steps (q unchanged, v = 0).
+// rows and records of a trajectory call (pk_rollout_trajectory_prepared).
 #pragma once
 
 #include "pk_coop.cuh"
@@ -44,19 +43,6 @@ __global__ void __launch_bounds__(kCoopThreads, CoopOccupancy<L>::min_blocks)
     else return P.joint[j];
   };
   GVar<typename Step::Lane, L> S;
-  // records of step s: the lane's joints of q and v, the status from lane 0 of the group
-  auto record = [&](int s, int st_all, bool frozen) {
-    const int64_t r = (int64_t)s * B + inst;
-#pragma unroll
-    for (int k = 0; k < NC; ++k) {
-      const int j = G.h * NC + k;
-      if (j < NJ) {
-        if (T.q) T.q[r * NJ + j] = S.v.q[k];
-        if (T.v) T.v[r * NJ + j] = frozen ? 0.f : S.v.x[k];
-      }
-    }
-    if (T.status && G.h == 0) T.status[r] = st_all;
-  };
   const float* qrow = q + inst * NJ;
   if constexpr (L == 1 && NJ % 2 == 0) {
 #pragma unroll
@@ -72,29 +58,8 @@ __global__ void __launch_bounds__(kCoopThreads, CoopOccupancy<L>::min_blocks)
       S.v.q[k] = (j < NJ) ? __ldg(qrow + (j < NJ ? j : 0)) : 0.f;
     }
   }
-  const float* trow = targets + inst * (int64_t)P.target_stride;
-  int st_all = 0;
-#pragma unroll
-  for (int k = 0; k < NC; ++k) S.v.x[k] = 0.f;
-#pragma unroll 1
-  for (int step_no = 0; step_no < n_steps; ++step_no) {
-    const bool frozen =
-        (st_all & (PK_STATUS_NO_SOLUTION | PK_STATUS_NOT_POSDEF)) || ((st_all & PK_STATUS_OUT_OF_LIMITS) && P.safety_break);
-    if (frozen) {
-#pragma unroll 1
-      for (int s = step_no; s < n_steps; ++s) record(s, st_all, true);
-      break;
-    }
-    int st;
-    ik_step_coop<NJ, NFT, L>(G, P, jc, trow, S, st);
-    st_all |= st & 0xff;
-    if (n_steps > 1 || q_out) {
-#pragma unroll
-      for (int k = 0; k < NC; ++k) S.v.q[k] = fmaf(S.v.x[k], P.dt, S.v.q[k]);  // 1-dof joints: q (+) v dt = q + v dt
-    }
-    trow += T.target_step;
-    record(step_no, st_all, false);
-  }
+  const int st_all = rollout_coop<NJ, NFT, L>(G, P, jc, targets + inst * (int64_t)P.target_stride, S, n_steps,
+                                              q_out != nullptr, T, B, inst);
   float* vrow = v + inst * NJ;
   if constexpr (L == 1 && NJ % 2 == 0) {
 #pragma unroll

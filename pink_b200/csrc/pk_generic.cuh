@@ -762,4 +762,32 @@ PK_HD void converge_generic(Generic<NJMAX, NVMAX>& G, const DevModel& M, const D
   status_out = st_all;
 }
 
+// Trajectory rollout of instance i on the general path (ik_generic_rollout_kernel): n_steps
+// iterations of Generic::step and q (+) v dt on q [nq] in place, the targets row of step s at
+// targets + s T.target_step + i target_stride, the records of T after every step.  An instance
+// whose statuses so far fail the freeze rule takes no further step (its records keep q, v = 0).
+// v [nv]: the last step's velocity.  Returns the OR of the statuses of the steps that ran.
+template <int NJMAX, int NVMAX>
+PK_HD int rollout_generic(Generic<NJMAX, NVMAX>& G, const DevModel& M, const DevProblem& P, float* q, float* v,
+                          const float* targets, int n_steps, const Trajectory& T, int64_t B, int64_t i) {
+  const int nq = M.nq, nv = M.nv;
+  int32_t st = 0;
+  GenericOut out{};
+  out.v = v;
+  out.status = &st;
+  out.task_index = -1;
+  int st_all = 0;
+  for (int s = 0; s < n_steps; ++s) {
+    if (step_failed(st_all, P.safety_break)) {
+      record_rows(T, s, B, i, nq, nv, q, v, st_all, true, 0, 1);
+      continue;
+    }
+    G.step(M, P, q, targets ? targets + s * T.target_step + i * (int64_t)P.target_stride : nullptr, out);
+    st_all |= st;
+    integrate_configuration(nq, M.free_flyer, q, v, P.dt, q);
+    record_rows(T, s, B, i, nq, nv, q, v, st_all, false, 0, 1);
+  }
+  return st_all;
+}
+
 }  // namespace pk

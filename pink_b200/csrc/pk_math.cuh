@@ -373,6 +373,17 @@ struct Trajectory {
   int32_t* status;      // [n_steps][B] OR of the statuses up to each step, or null
 };
 
+// Records of step s of a trajectory from an instance's q / v rows (`n` threads from `lane`).
+PK_HD void record_rows(const Trajectory& T, int s, int64_t B, int64_t i, int nq, int nv, const float* qrow,
+                       const float* vrow, int st_all, bool frozen, int lane, int n) {
+  const int64_t r = (int64_t)s * B + i;
+  if (T.q)
+    for (int k = lane; k < nq; k += n) T.q[r * nq + k] = qrow[k];
+  if (T.v)
+    for (int k = lane; k < nv; k += n) T.v[r * nv + k] = frozen ? 0.f : vrow[k];
+  if (T.status && lane == 0) T.status[r] = st_all;
+}
+
 // The freeze rule of the rollouts: an instance whose statuses so far have one of these bits
 // takes no further step.
 PK_HD bool step_failed(int st_all, int safety_break) {

@@ -1200,6 +1200,36 @@ struct TreeStep {
     steps = s;
     status_out = st_all;
   }
+
+  // Closed-loop rollout of instance i, one instance per warp (ik_tree_rollout_kernel): n_steps
+  // iterations of run and q (+) v dt on qg [nq] in place (by lane 0), the targets row of step s at
+  // targets + s T.target_step + i L.stride, the records of T after every step.  A step that fails
+  // the freeze rule is recorded without moving q and ends the loop; the remaining steps are
+  // recorded with q unchanged and v = 0.  vg [nv]: the last step's velocity.  Returns the OR of
+  // the statuses of the steps that ran, the same on every lane.
+  static PK_HD int rollout(const DevModel& M, const DevProblem& P, const TreePlan& L, float* qg, const float* targets,
+                           float* W, float* vg, int n_steps, const Trajectory& T, int64_t B, int64_t i) {
+    int st_all = 0;
+    int s = 0;
+    while (s < n_steps) {
+      int32_t st = 0;
+      run(M, P, L, qg, targets ? targets + s * T.target_step + i * (int64_t)L.stride : nullptr, W, vg, &st);
+      PK_WSYNC();
+      st = lane0_int(st);  // run() reports through lane 0
+      st_all |= st;
+      const bool failed = step_failed(st, P.safety_break);
+      PK_LANES(l) {
+        if (!failed && l == 0) integrate_configuration(L.nq, M.free_flyer, qg, vg, P.dt, qg);
+      }
+      PK_WSYNC();
+      const int recorded = s++;  // advanced before the stores: 4 B fewer spill loads than after them
+      PK_LANES(l) record_rows(T, recorded, B, i, L.nq, L.nv, qg, vg, st_all, false, l, 32);
+      if (failed) break;
+    }
+    for (; s < n_steps; ++s)
+      PK_LANES(l) record_rows(T, s, B, i, L.nq, L.nv, qg, vg, st_all, true, l, 32);
+    return st_all;
+  }
 };
 
 }  // namespace pk

@@ -90,6 +90,8 @@ __device__ __forceinline__ int lane_or(const LaneVar<int>& a) {
 __device__ __forceinline__ float lane_bcast(const LaneVar<float>& a, int src) {
   return __shfl_sync(0xffffffffu, a.v, src);
 }
+// lane 0's x, on every lane (on the host x is the one value lane 0 wrote)
+__device__ __forceinline__ int lane0_int(int x) { return __shfl_sync(0xffffffffu, x, 0); }
 __device__ __forceinline__ double lane_sum_d(const LaneVar<double>& a) {
   double s = a.v;
 #pragma unroll
@@ -140,6 +142,7 @@ inline int lane_or(const LaneVar<int>& a) {
   return s;
 }
 inline float lane_bcast(const LaneVar<float>& a, int src) { return a.v[src]; }
+inline int lane0_int(int x) { return x; }
 inline double lane_sum_d(const LaneVar<double>& a) {
   double t[32];
   for (int l = 0; l < 32; ++l) t[l] = a.v[l];

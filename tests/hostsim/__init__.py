@@ -1,5 +1,6 @@
 """ctypes wrapper of ``libpk_hostsim.so``: the kernel bodies of
-``pink_b200/csrc`` compiled for the host CPU (see hostsim.cpp).
+``pink_b200/csrc`` and their rollout, converge and multi-start loops compiled for the host CPU
+(see hostsim.cpp).
 
 TEST HARNESS ONLY.  The product package never imports this module; it exists
 so that the CPU test-suite can run the kernels' exact fp32 arithmetic against
@@ -61,6 +62,11 @@ def _p(a):
 Selection = namedtuple("Selection", "path nj nft generic lanes pdl_row_fits K")
 
 
+def _selection(sel):
+    return Selection(("chain", "tree", "general")[sel[0]], sel[1], sel[2], (sel[3], sel[4]), sel[5], bool(sel[6]),
+                     sel[7])
+
+
 class HostSim:
     """Runs the kernel bodies on the CPU for one model."""
 
@@ -102,9 +108,69 @@ class HostSim:
         sel = (C.c_int * 8)()
         self._chk(lib().hs_solve_ik(self.handle, C.byref(prob), _p(q), _p(t), _p(v), _p(st),
                                     C.c_int64(B), (1 if general_path else 0) if path is None else path, sel))
-        self.selection = Selection(("chain", "tree", "general")[sel[0]], sel[1], sel[2], (sel[3], sel[4]), sel[5],
-                                   bool(sel[6]), sel[7])
+        self.selection = _selection(sel)
         return v, st
+
+    def rollout(self, prob, q, targets, n_steps, target_step=None, record=True, path=0):
+        """Trajectory rollout with the loop of the selected body (hs_rollout): ``targets`` is
+        ``[n_steps, B, stride]`` (step s at ``target_step`` floats from step 0; default: its stride)
+        or ``[B, stride]`` (the same rows every step, ``target_step`` 0).  Returns ``(q, v, status,
+        q_traj, v_traj, status_traj)``, the records None unless ``record``; ``path`` as
+        :meth:`solve_ik`."""
+        q = self._f32(q)
+        B = q.shape[0]
+        t = None if targets is None else np.asarray(targets, dtype=np.float32)
+        if t is not None and t.ndim < 3:
+            t = self._f32(t)
+        if target_step is None:
+            target_step = t.strides[0] // 4 if t is not None and t.ndim == 3 else 0
+        q_out = np.zeros_like(q)
+        v = np.zeros((B, self.nv), dtype=np.float32)
+        st = np.zeros(B, dtype=np.int32)
+        rec = ((np.zeros((n_steps, B, self.nq), dtype=np.float32), np.zeros((n_steps, B, self.nv), dtype=np.float32),
+                np.zeros((n_steps, B), dtype=np.int32)) if record else (None, None, None))
+        sel = (C.c_int * 8)()
+        self._chk(lib().hs_rollout(self.handle, C.byref(prob), _p(q), _p(t), C.c_int64(target_step), n_steps,
+                                   _p(q_out), _p(v), _p(st), *map(_p, rec), C.c_int64(B), path, sel))
+        self.selection = _selection(sel)
+        return (q_out, v, st) + rec
+
+    def converge(self, prob, q, targets, mask, tol, max_steps, path=0):
+        """Solve to a tolerance with the converge loop of the selected body (hs_converge):
+        ``(q_out, err, steps, status)``; ``path`` as :meth:`solve_ik`, and ``self.selection``
+        the kernel selection the loop ran."""
+        q = self._f32(q)
+        B = q.shape[0]
+        t = None if targets is None else self._f32(targets)
+        q_out = np.zeros_like(q)
+        err = np.zeros(B, dtype=np.float32)
+        steps = np.zeros(B, dtype=np.int32)
+        st = np.zeros(B, dtype=np.int32)
+        sel = (C.c_int * 8)()
+        self._chk(lib().hs_converge(self.handle, C.byref(prob), _p(q), _p(t), C.c_uint32(mask), C.c_float(tol),
+                                    C.c_int(max_steps), _p(q_out), _p(err), _p(steps), _p(st), C.c_int64(B), path,
+                                    sel))
+        self.selection = _selection(sel)
+        return q_out, err, steps, st
+
+    def converge_multistart(self, prob, q_seeds, targets, mask, tol, max_steps, path=0):
+        """Multi-start solve to a tolerance (hs_converge_multistart): ``q_seeds [B, S, nq]`` ->
+        ``(q_out, err, seed, steps, status)``; ``path`` as :meth:`solve_ik` (0: the library's
+        selection, 1: the general path, 2: the tree kernel)."""
+        qs = self._f32(q_seeds)
+        B, S, nq = qs.shape
+        t = None if targets is None else self._f32(targets)
+        q_out = np.zeros((B, nq), dtype=np.float32)
+        err = np.zeros(B, dtype=np.float32)
+        seed = np.zeros(B, dtype=np.int32)
+        steps = np.zeros(B, dtype=np.int32)
+        st = np.zeros(B, dtype=np.int32)
+        sel = (C.c_int * 8)()
+        self._chk(lib().hs_converge_multistart(self.handle, C.byref(prob), _p(qs), S, _p(t), C.c_uint32(mask),
+                                               C.c_float(tol), C.c_int(max_steps), _p(q_out), _p(err), _p(seed),
+                                               _p(steps), _p(st), C.c_int64(B), path, sel))
+        self.selection = _selection(sel)
+        return q_out, err, seed, steps, st
 
     @property
     def used_chain(self):

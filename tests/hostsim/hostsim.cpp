@@ -1,8 +1,9 @@
-// CPU build of the kernel bodies (pk_chain.cuh / pk_generic.cuh) for the test
-// suite ONLY: lets `pytest -m "not gpu"` exercise the exact fp32 arithmetic and
+// CPU build of the kernel bodies (pk_chain.cuh / pk_generic.cuh) for the test suite
+// ONLY: lets `pytest -m "not gpu"` exercise the exact fp32 arithmetic and
 // control flow of the CUDA kernels against the fp64 oracle on machines without
 // a GPU.  It is never loaded by the product package (pink_b200/_cabi.py loads
 // libpink_b200.so and nothing else) and is not a fallback.
+#include <cmath>
 #include <cstdint>
 #include <cstring>
 #include <string>
@@ -16,13 +17,80 @@ namespace {
 thread_local std::string g_err;
 int fail(const std::string& m) { g_err = m; return 1; }
 
-// The bodies of the kernels a chain selection names, lanes emulated by loops in the sub-warp one.
-template <int NJ, int NFT>
-void run_chain(const pk::HostModel& hm, const pk::DevProblem& P, const pk::Selection& sel, const float* q,
-               const float* targets, float* v, int32_t* status, int64_t B) {
+// make_dev_problem + host image of the optional parts, wired through P.ext
+std::string make_problem(const pk::HostModel& hm, const PkProblemDesc* prob, pk::DevProblem* P, pk::HostExtras* hx) {
+  const std::string e = pk::make_dev_problem(hm, prob, P, hx);
+  if (e.empty() && hx->present) P->ext = &hx->X;
+  return e;
+}
+
+// The CUDA library's kernel selection (pk_select.hpp) for `path`: 0 the library's default options,
+// 1 PK_FORCE_GENERIC=1, 2 without the chain kernels (the tree kernel body on a chain),
+// 11 / 12 / 14 / 18 PK_CHAIN_LANES = 1 / 2 / 4 / 8 (the problem must take a chain kernel) when
+// `sub_warp`, the tree kernel or the general path otherwise.  sel_out: path (pk::KernelPath), nj,
+// nft, the general path's <NJMAX, NVMAX>, lanes, PDL row fits, tree task rows K.  Returns the
+// error of a path the problem does not fit, or "".
+std::string select(const pk::HostModel& hm, const pk::DevProblem& P, const pk::HostExtras& hx, int path,
+                   bool sub_warp, int* sel_out, pk::Selection* sel) {
+  const bool lanes = sub_warp && path > 10;
+  pk::SelectOptions o;
+  o.use_chain = path == 0 || lanes;
+  o.use_tree = path != 1;
+  o.chain_lanes = lanes ? path - 10 : 0;
+  const pk::Selection& s = *sel = pk::select_kernel(hm, P, hx, o);
+  const int report[] = {s.path, s.nj, s.nft, 0, 0, s.lanes, s.pdl_row_fits, s.plan.K};
+  std::memcpy(sel_out, report, sizeof(report));
+  pk::with_generic(s.generic_class, [&](auto nj, auto nv) { sel_out[3] = nj; sel_out[4] = nv; });
+  if (lanes && s.path != pk::kPathChain) return "problem does not fit the chain kernel";
+  if (path == 2 && s.path != pk::kPathTree) return "problem does not fit the tree kernel";
+  return "";
+}
+
+// A tree kernel's workspace of `words` floats in W, 8-byte aligned: the dual method keeps doubles in it.
+float* tree_workspace(std::vector<float>& W, int words) {
+  W.assign(words + 8, 0.f);
+  float* p = W.data();
+  return ((uintptr_t)p & 7) != 0 ? p + 1 : p;
+}
+
+// The chain kernel a chain selection names: chain(C) with the thread-per-instance kernel's
+// parameter block, or coop(lanes, C, jc) with the sub-warp kernel's (lanes emulated by loops).
+template <int NJ, int NFT, class Chain, class Coop>
+void with_chain_kernel(const pk::HostModel& hm, const pk::DevProblem& P, const pk::Selection& sel, Chain chain,
+                       Coop coop) {
   if (!sel.lanes) {
     pk::ChainParams<NJ> C;
     pk::make_chain_params<NJ>(hm, P, &C, P.ext);
+    return chain(C);
+  }
+  pk::with_lanes<NJ, NFT>(sel.lanes, [&](auto lanes) {
+    typename pk::CoopStep<NJ, NFT, decltype(lanes)::value>::Params C;
+    pk::make_coop_params<NJ, decltype(lanes)::value>(hm, P, &C, P.ext);
+    coop(lanes, C, [&](int j) -> const pk::CoopJoint& { return C.joint[j]; });
+  });
+}
+
+// Instance i's q row into the lanes of the sub-warp kernel (padding joints at zero), and back:
+// the lanes' q into q_out row i (unless null) and their velocity into v row i.
+template <int NJ, int NC, int L, class Lane>
+void coop_load(pk::GVar<Lane, L>& S, const float* q, int64_t i) {
+  for (int h = 0; h < L; ++h)
+    for (int k = 0; k < NC; ++k) S[h].q[k] = h * NC + k < NJ ? q[i * NJ + h * NC + k] : 0.f;
+}
+template <int NJ, int NC, int L, class Lane>
+void coop_store(const pk::GVar<Lane, L>& S, float* q_out, float* v, int64_t i) {
+  for (int h = 0; h < L; ++h)
+    for (int k = 0; k < NC && h * NC + k < NJ; ++k) {
+      if (q_out) q_out[i * NJ + h * NC + k] = S[h].q[k];
+      v[i * NJ + h * NC + k] = S[h].x[k];
+    }
+}
+
+// The bodies of the kernels a chain selection names.
+template <int NJ, int NFT>
+void run_chain(const pk::HostModel& hm, const pk::DevProblem& P, const pk::Selection& sel, const float* q,
+               const float* targets, float* v, int32_t* status, int64_t B) {
+  auto chain = [&](const pk::ChainParams<NJ>& C) {
     for (int64_t i = 0; i < B; ++i) {
       float qi[NJ], vi[NJ];
       for (int k = 0; k < NJ; ++k) qi[k] = q[i * NJ + k];
@@ -31,39 +99,20 @@ void run_chain(const pk::HostModel& hm, const pk::DevProblem& P, const pk::Selec
       for (int k = 0; k < NJ; ++k) v[i * NJ + k] = vi[k];
       if (status) status[i] = st;
     }
-    return;
-  }
-  pk::with_lanes<NJ, NFT>(sel.lanes, [&](auto lanes) {
+  };
+  auto coop = [&](auto lanes, const auto& C, auto jc) {
     constexpr int L = decltype(lanes)::value;
     using Step = pk::CoopStep<NJ, NFT, L>;
-    typename Step::Params C;
-    pk::make_coop_params<NJ, L>(hm, P, &C, P.ext);
-    const pk::Group<L> G{};
-    auto jc = [&](int j) -> const pk::CoopJoint& { return C.joint[j]; };
     for (int64_t i = 0; i < B; ++i) {
       pk::GVar<typename Step::Lane, L> S;
-      for (int h = 0; h < L; ++h)
-        for (int k = 0; k < Step::NC; ++k) {
-          const int j = h * Step::NC + k;
-          S[h].q[k] = j < NJ ? q[i * NJ + j] : 0.f;
-        }
+      coop_load<NJ, Step::NC>(S, q, i);
       int st = 0;
-      pk::ik_step_coop<NJ, NFT, L>(G, C, jc, targets + i * (int64_t)P.target_stride, S, st);
-      for (int h = 0; h < L; ++h)
-        for (int k = 0; k < Step::NC; ++k) {
-          const int j = h * Step::NC + k;
-          if (j < NJ) v[i * NJ + j] = S[h].x[k];
-        }
+      pk::ik_step_coop<NJ, NFT, L>(pk::Group<L>{}, C, jc, targets + i * (int64_t)P.target_stride, S, st);
+      coop_store<NJ, Step::NC>(S, nullptr, v, i);
       if (status) status[i] = st;
     }
-  });
-}
-
-// make_dev_problem + host image of the optional parts, wired through P.ext
-std::string make_problem(const pk::HostModel& hm, const PkProblemDesc* prob, pk::DevProblem* P, pk::HostExtras* hx) {
-  const std::string e = pk::make_dev_problem(hm, prob, P, hx);
-  if (e.empty() && hx->present) P->ext = &hx->X;
-  return e;
+  };
+  with_chain_kernel<NJ, NFT>(hm, P, sel, chain, coop);
 }
 
 // ik_generic_kernel's body at the instantiation the CUDA library launches for this model
@@ -75,6 +124,30 @@ void run_generic(const pk::HostModel& hm, const pk::DevProblem& P, const pk::Gen
       G.step(M, P, A.q + i * M.nq, A.targets ? A.targets + i * (int64_t)P.target_stride : nullptr,
              pk::generic_out(M, A, i));
   });
+}
+
+// One multi-start group of S seeds.  error(j) -> err(q_j); advance(j) -> the step of seed j, false
+// when it fails (q_j unchanged), its status ORed into st_all[j].  Returns the winner; e, steps out.
+template <class Error, class Advance>
+int run_group(int S, float tol, int max_steps, Error error, Advance advance, std::vector<float>& e, int& steps) {
+  std::vector<char> failed(S, 0);
+  int s = 0;
+  for (;; ++s) {
+    bool hit = false, all_failed = true;
+    for (int j = 0; j < S; ++j) {
+      if (!failed[j]) e[j] = error(j);
+      hit = hit || e[j] <= tol;
+      all_failed = all_failed && failed[j];
+    }
+    if (hit || s == max_steps || all_failed) break;
+    for (int j = 0; j < S; ++j)
+      if (!failed[j] && !advance(j)) failed[j] = 1;
+  }
+  steps = s;
+  int w = 0;
+  for (int j = 1; j < S; ++j)
+    if (pk::seed_before(e[j], j, e[w], w)) w = j;
+  return w;
 }
 }  // namespace
 
@@ -91,11 +164,7 @@ int hs_model_create(const PkModelDesc* d, void** out) {
 }
 void hs_model_destroy(void* m) { delete (pk::HostModel*)m; }
 
-// The kernel body the CUDA library's selection (pk_select.hpp) names for this problem.
-// path: 0 the library's default options, 1 PK_FORCE_GENERIC=1, 2 without the chain kernels (the
-// tree kernel body on a chain), 11 / 12 / 14 / 18 PK_CHAIN_LANES = 1 / 2 / 4 / 8 (the problem must
-// take a chain kernel).  sel_out: path (pk::KernelPath), nj, nft, the general path's <NJMAX, NVMAX>,
-// lanes, PDL row fits, tree task rows K.
+// The kernel body the CUDA library's selection names for this problem; path and sel_out: see select.
 int hs_solve_ik(void* model, const PkProblemDesc* prob, const float* q, const float* targets, float* v,
                 int32_t* status, int64_t B, int path, int* sel_out) {
   const pk::HostModel& hm = *(pk::HostModel*)model;
@@ -103,16 +172,9 @@ int hs_solve_ik(void* model, const PkProblemDesc* prob, const float* q, const fl
   pk::HostExtras hx;
   const std::string e = make_problem(hm, prob, &P, &hx);
   if (!e.empty()) return fail(e);
-  pk::SelectOptions o;
-  o.use_chain = path == 0 || path > 10;
-  o.use_tree = path != 1;
-  o.chain_lanes = path > 10 ? path - 10 : 0;
-  const pk::Selection sel = pk::select_kernel(hm, P, hx, o);
-  const int report[] = {sel.path, sel.nj, sel.nft, 0, 0, sel.lanes, sel.pdl_row_fits, sel.plan.K};
-  std::memcpy(sel_out, report, sizeof(report));
-  pk::with_generic(sel.generic_class, [&](auto nj, auto nv) { sel_out[3] = nj; sel_out[4] = nv; });
-  if (path > 10 && sel.path != pk::kPathChain) return fail("problem does not fit the chain kernel");
-  if (path == 2 && sel.path != pk::kPathTree) return fail("problem does not fit the tree kernel");
+  pk::Selection sel;
+  const std::string serr = select(hm, P, hx, path, true, sel_out, &sel);
+  if (!serr.empty()) return fail(serr);
   if (sel.path == pk::kPathChain) {
     pk::with_nj(sel.nj, [&](auto nj) {
       pk::with_nft(sel.nft, [&](auto nft) {
@@ -122,9 +184,8 @@ int hs_solve_ik(void* model, const PkProblemDesc* prob, const float* q, const fl
   } else if (sel.path == pk::kPathTree) {
     const pk::TreePlan& L = sel.plan;
     const pk::DevModel M = hm.host_view();
-    std::vector<float> W(L.words + 8);
-    float* Wp = W.data();
-    if (((uintptr_t)Wp & 7) != 0) ++Wp;  // the dual method keeps doubles in the workspace
+    std::vector<float> W;
+    float* Wp = tree_workspace(W, L.words);
     for (int64_t i = 0; i < B; ++i)
       pk::TreeStep::run(M, P, L, q + i * L.nq, targets ? targets + i * (int64_t)L.stride : nullptr, Wp,
                         v + i * L.nv, status ? status + i : nullptr);
@@ -132,6 +193,263 @@ int hs_solve_ik(void* model, const PkProblemDesc* prob, const float* q, const fl
     pk::GenericArgs A{};
     A.q = q; A.targets = targets; A.v = v; A.status = status; A.task_index = -1;
     run_generic(hm, P, A, B);
+  }
+  return 0;
+}
+
+// Trajectory rollout (pk_rollout_trajectory_prepared) with the loop of the body the selection names:
+// rollout_chain, rollout_coop (path 11 / 12 / 14 / 18), TreeStep::rollout or rollout_generic.
+// targets [B][target_stride] for step 0, step s target_step floats further; q_traj / v_traj /
+// status_traj: the step-major records, or null.  path and sel_out as hs_solve_ik.
+int hs_rollout(void* model, const PkProblemDesc* prob, const float* q, const float* targets, int64_t target_step,
+               int n_steps, float* q_out, float* v, int32_t* status, float* q_traj, float* v_traj,
+               int32_t* status_traj, int64_t B, int path, int* sel_out) {
+  const pk::HostModel& hm = *(pk::HostModel*)model;
+  pk::DevProblem P;
+  pk::HostExtras hx;
+  const std::string e = make_problem(hm, prob, &P, &hx);
+  if (!e.empty()) return fail(e);
+  pk::Selection sel;
+  const std::string serr = select(hm, P, hx, path, true, sel_out, &sel);
+  if (!serr.empty()) return fail(serr);
+  const pk::Trajectory T{target_step, q_traj, v_traj, status_traj};
+  const pk::DevModel M = hm.host_view();
+  const int nq = hm.nq, nv = hm.nv;
+  auto start = [&](int64_t i) {
+    float* qrow = q_out + i * nq;
+    std::memcpy(qrow, q + i * nq, sizeof(float) * nq);
+    return qrow;
+  };
+  if (sel.path == pk::kPathChain) {
+    pk::with_nj(sel.nj, [&](auto nj) {
+      constexpr int NJ = decltype(nj)::value;
+      pk::with_nft(sel.nft, [&](auto nft) {
+        constexpr int NFT = decltype(nft)::value;
+        auto chain = [&](const pk::ChainParams<NJ>& C) {
+          for (int64_t i = 0; i < B; ++i) {
+            float qi[NJ], vi[NJ];
+            for (int k = 0; k < NJ; ++k) qi[k] = q[i * NJ + k];
+            const int st_all = pk::rollout_chain<NJ, NFT, true>(C, qi, targets + i * (int64_t)P.target_stride, vi,
+                                                                n_steps, true, 0, T, B, i);
+            for (int k = 0; k < NJ; ++k) { q_out[i * NJ + k] = qi[k]; v[i * NJ + k] = vi[k]; }
+            if (status) status[i] = st_all;
+          }
+        };
+        auto coop = [&](auto lanes, const auto& C, auto jc) {
+          constexpr int L = decltype(lanes)::value;
+          using Step = pk::CoopStep<NJ, NFT, L>;
+          for (int64_t i = 0; i < B; ++i) {
+            pk::GVar<typename Step::Lane, L> S;
+            coop_load<NJ, Step::NC>(S, q, i);
+            const int st_all = pk::rollout_coop<NJ, NFT, L>(pk::Group<L>{}, C, jc,
+                                                            targets + i * (int64_t)P.target_stride, S, n_steps, true,
+                                                            T, B, i);
+            coop_store<NJ, Step::NC>(S, q_out, v, i);
+            if (status) status[i] = st_all;
+          }
+        };
+        with_chain_kernel<NJ, NFT>(hm, P, sel, chain, coop);
+      });
+    });
+  } else if (sel.path == pk::kPathTree) {
+    std::vector<float> W;
+    float* Wp = tree_workspace(W, sel.plan.words);
+    for (int64_t i = 0; i < B; ++i) {
+      const int st_all = pk::TreeStep::rollout(M, P, sel.plan, start(i), targets, Wp, v + i * nv, n_steps, T, B, i);
+      if (status) status[i] = st_all;
+    }
+  } else {
+    pk::with_generic(sel.generic_class, [&](auto nj, auto nvm) {
+      static thread_local pk::Generic<decltype(nj)::value, decltype(nvm)::value> G;
+      for (int64_t i = 0; i < B; ++i) {
+        const int st_all = pk::rollout_generic(G, M, P, start(i), v + i * nv, targets, n_steps, T, B, i);
+        if (status) status[i] = st_all;
+      }
+    });
+  }
+  return 0;
+}
+
+// Solve to a tolerance (pk_converge_prepared) with the converge loop of the body the selection
+// names: converge_chain (always the thread-per-instance kernel), TreeStep::converge or
+// converge_generic.  path and sel_out as hs_solve_ik.  q_out may alias q.
+int hs_converge(void* model, const PkProblemDesc* prob, const float* q, const float* targets, uint32_t mask,
+                float tol, int max_steps, float* q_out, float* err, int32_t* steps, int32_t* status, int64_t B,
+                int path, int* sel_out) {
+  const pk::HostModel& hm = *(pk::HostModel*)model;
+  pk::DevProblem P;
+  pk::HostExtras hx;
+  const std::string e = make_problem(hm, prob, &P, &hx);
+  if (!e.empty()) return fail(e);
+  const std::string aerr = pk::check_converge_args(P, mask, tol, max_steps);
+  if (!aerr.empty()) return fail(aerr);
+  if (B > 0 && P.target_stride > 0 && !targets) return fail("null targets");
+  pk::Selection sel;
+  const std::string serr = select(hm, P, hx, path, true, sel_out, &sel);
+  if (!serr.empty()) return fail(serr);
+  const pk::DevModel M = hm.host_view();
+  const int nq = hm.nq;
+  auto trow = [&](int64_t i) { return targets ? targets + i * (int64_t)P.target_stride : nullptr; };
+  auto start = [&](int64_t i) {
+    float* qrow = q_out + i * nq;
+    if (qrow != q + i * nq) std::memcpy(qrow, q + i * nq, sizeof(float) * nq);
+    return qrow;
+  };
+  auto store = [&](int64_t i, float ei, int n, int st) {
+    if (err) err[i] = ei;
+    if (steps) steps[i] = n;
+    if (status) status[i] = st;
+  };
+  float ei;
+  int n, st;
+  if (sel.path == pk::kPathChain) {
+    pk::with_nj(sel.nj, [&](auto nj) {
+      constexpr int NJ = decltype(nj)::value;
+      pk::ChainParams<NJ> C;
+      pk::make_chain_params<NJ>(hm, P, &C, P.ext);
+      const unsigned emask = pk::chain_task_mask(P, mask, sel.nft);
+      pk::with_nft(sel.nft, [&](auto nft) {
+        for (int64_t i = 0; i < B; ++i) {
+          float qi[NJ];
+          for (int k = 0; k < NJ; ++k) qi[k] = q[i * NJ + k];
+          pk::converge_chain<NJ, decltype(nft)::value>(C, qi, trow(i), emask, tol, max_steps, ei, n, st);
+          for (int k = 0; k < NJ; ++k) q_out[i * NJ + k] = qi[k];
+          store(i, ei, n, st);
+        }
+      });
+    });
+  } else if (sel.path == pk::kPathTree) {
+    std::vector<float> W, v(hm.nv);
+    float* Wp = tree_workspace(W, sel.plan.words);
+    for (int64_t i = 0; i < B; ++i) {
+      pk::TreeStep::converge(M, P, sel.plan, start(i), trow(i), Wp, v.data(), mask, tol, max_steps, ei, n, st);
+      store(i, ei, n, st);
+    }
+  } else {
+    pk::with_generic(sel.generic_class, [&](auto nj, auto nv) {
+      static thread_local pk::Generic<decltype(nj)::value, decltype(nv)::value> G;
+      float v[decltype(nv)::value];
+      for (int64_t i = 0; i < B; ++i) {
+        pk::converge_generic(G, M, P, start(i), trow(i), v, mask, tol, max_steps, ei, n, st);
+        store(i, ei, n, st);
+      }
+    });
+  }
+  return 0;
+}
+
+// Multi-start solve to a tolerance (pk_converge_multistart_prepared) with the bodies the selection
+// names; q_seeds [B S][nq], the outputs [B].  path as hs_converge without the sub-warp kernel.
+// A host thread cannot suspend inside a step body to wait for the other seeds of its group, so
+// each round runs in two passes over the group: first every seed's error, from the step body
+// with its stop forced (it returns before the QP); then the group's decision, and the step of
+// every seed that goes on.  The bodies (ChainStep::assemble<true> with converge_chain_advance,
+// TreeStep::run<true>, Generic::step<true>) and the winner's order (seed_before) are those the
+// CUDA library runs.
+int hs_converge_multistart(void* model, const PkProblemDesc* prob, const float* q_seeds, int S,
+                           const float* targets, uint32_t mask, float tol, int max_steps, float* q_out, float* err,
+                           int32_t* seed, int32_t* steps, int32_t* status, int64_t B, int path, int* sel_out) {
+  const pk::HostModel& hm = *(pk::HostModel*)model;
+  pk::DevProblem P;
+  pk::HostExtras hx;
+  const std::string e = make_problem(hm, prob, &P, &hx);
+  if (!e.empty()) return fail(e);
+  const std::string aerr = pk::check_converge_args(P, mask, tol, max_steps);
+  if (!aerr.empty()) return fail(aerr);
+  pk::Selection sel;
+  const std::string serr = select(hm, P, hx, path, false, sel_out, &sel);
+  if (!serr.empty()) return fail(serr);
+  const std::string kerr = pk::check_multistart_seeds(sel, S);
+  if (!kerr.empty()) return fail(kerr);
+  if (B > 0 && P.target_stride > 0 && !targets) return fail("null targets");
+  const pk::DevModel M = hm.host_view();
+  const int nq = hm.nq;
+  // the forced stop of the first pass, and the test of the second (never stops: err >= 0)
+  const pk::ConvergeTest probe{mask, tol, true, 0.f, false, 0};
+  const pk::ConvergeTest go{mask, -INFINITY, false, 0.f, false, 0};
+  std::vector<float> qs((size_t)S * nq), es(S);
+  std::vector<int> st_all(S);
+  for (int64_t b = 0; b < B; ++b) {
+    const float* trow = targets ? targets + b * (int64_t)P.target_stride : nullptr;
+    std::memcpy(qs.data(), q_seeds + b * S * nq, sizeof(float) * S * nq);
+    std::fill(st_all.begin(), st_all.end(), 0);
+    int w = 0, n = 0;
+    if (sel.path == pk::kPathChain) {
+      pk::with_nj(sel.nj, [&](auto nj) {
+        constexpr int NJ = decltype(nj)::value;
+        pk::ChainParams<NJ> C;
+        pk::make_chain_params<NJ>(hm, P, &C, P.ext);
+        const unsigned emask = pk::chain_task_mask(P, mask, sel.nft);
+        pk::with_nft(sel.nft, [&](auto nft) {
+          constexpr int NFT = decltype(nft)::value;
+          auto qj = [&](int j) -> float(&)[NJ] { return *reinterpret_cast<float(*)[NJ]>(qs.data() + j * NJ); };
+          auto error = [&](int j) {
+            pk::ChainStep<NJ, NFT> Cs;
+            bool skip;
+            float ej;
+            Cs.template assemble<true>(C, qj(j), trow, skip, emask, &ej);
+            return ej;
+          };
+          auto advance = [&](int j) {
+            pk::ChainStep<NJ, NFT> Cs;
+            bool skip;
+            float ej;
+            const int st = Cs.template assemble<true>(C, qj(j), trow, skip, emask, &ej);
+            return pk::converge_chain_advance(C, Cs, st, skip, qj(j), st_all[j], 0);
+          };
+          w = run_group(S, tol, max_steps, error, advance, es, n);
+        });
+      });
+    } else if (sel.path == pk::kPathTree) {
+      const pk::TreePlan& L = sel.plan;
+      std::vector<float> W, v(hm.nv);
+      float* Wp = tree_workspace(W, L.words);
+      auto error = [&](int j) {
+        pk::ConvergeTest ct = probe;
+        pk::TreeStep::run<true>(M, P, L, qs.data() + j * nq, trow, Wp, v.data(), nullptr, &ct);
+        return ct.err;
+      };
+      auto advance = [&](int j) {
+        float* q = qs.data() + j * nq;
+        pk::ConvergeTest ct = go;
+        pk::TreeStep::run<true>(M, P, L, q, trow, Wp, v.data(), nullptr, &ct);
+        st_all[j] |= ct.status;
+        if (pk::step_failed(st_all[j], P.safety_break)) return false;
+        pk::integrate_configuration(nq, M.free_flyer, q, v.data(), P.dt, q);
+        return true;
+      };
+      w = run_group(S, tol, max_steps, error, advance, es, n);
+    } else {
+      pk::with_generic(sel.generic_class, [&](auto nj, auto nv) {
+        static thread_local pk::Generic<decltype(nj)::value, decltype(nv)::value> G;
+        float v[decltype(nv)::value];
+        int32_t st = 0;
+        pk::GenericOut out{};
+        out.v = v;
+        out.status = &st;
+        out.task_index = -1;
+        auto error = [&](int j) {
+          pk::ConvergeTest ct = probe;
+          G.template step<true>(M, P, qs.data() + j * nq, trow, out, &ct);
+          return ct.err;
+        };
+        auto advance = [&](int j) {
+          float* q = qs.data() + j * nq;
+          pk::ConvergeTest ct = go;
+          G.template step<true>(M, P, q, trow, out, &ct);
+          st_all[j] |= st;
+          if (pk::step_failed(st_all[j], P.safety_break)) return false;
+          pk::integrate_configuration(nq, M.free_flyer, q, v, P.dt, q);
+          return true;
+        };
+        w = run_group(S, tol, max_steps, error, advance, es, n);
+      });
+    }
+    std::memcpy(q_out + b * nq, qs.data() + w * nq, sizeof(float) * nq);
+    if (err) err[b] = es[w];
+    if (seed) seed[b] = w;
+    if (steps) steps[b] = n;
+    if (status) status[b] = st_all[w];
   }
   return 0;
 }
@@ -230,9 +548,8 @@ int hs_tree_dual_qp(int K, int n, int p, int meq, const float* A, const float* b
   memset(&L, 0, sizeof(L));
   L.nj = 1; L.nq = n; L.nv = n; L.K = K; L.p = p; L.meq = meq; L.npairs = 0;
   pk::tree_layout(L, 1, 0);
-  std::vector<float> W(L.words + 8, 0.f);
-  float* Wp = W.data();
-  if (((uintptr_t)Wp & 7) != 0) ++Wp;  // doubles in the workspace
+  std::vector<float> W;
+  float* Wp = tree_workspace(W, L.words);
   for (int r = 0; r < K; ++r) {
     for (int c = 0; c < n; ++c) Wp[L.o_A + r * L.lda + c] = A[r * n + c];
     Wp[L.o_b + r] = b[r];

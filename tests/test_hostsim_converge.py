@@ -15,7 +15,7 @@ from oracle import kinematics as okin
 from oracle import tasks as otasks
 from pink_b200 import _cabi
 from tests import extras, helpers
-from tests.hostsim.converge import ConvergeSim
+from tests.hostsim import HostSim
 
 FAILED = _cabi.PK_STATUS_NO_SOLUTION | _cabi.PK_STATUS_NOT_POSDEF
 
@@ -85,7 +85,7 @@ def check(sc, mask, tol, max_steps, path=0, expect=None, q=None, targets=None, n
     prob, tg, _ = sc.problem()
     targets = tg if targets is None else targets
     q = sc.q32 if q is None else q
-    hs = ConvergeSim(sc.model)
+    hs = HostSim(sc.model)
     q_out, err, steps, st = hs.converge(prob, q, targets, mask, tol, max_steps, path=path)
     if expect is not None:
         assert hs.selection.path == expect, hs.selection
@@ -182,7 +182,7 @@ def test_general_path_tree_extras_40_joints():
 def test_tol_met_at_start_and_zero_max_steps():
     sc = helpers.ur5_scenario(16, "at_target")
     prob, targets, _ = sc.problem()
-    hs = ConvergeSim(sc.model)
+    hs = HostSim(sc.model)
     q_out, err, steps, st = hs.converge(prob, sc.q32, targets, 0b01, 1e-4, 50)
     assert (steps == 0).all() and (st == 0).all() and (err <= 1e-4).all()
     np.testing.assert_array_equal(q_out.view(np.int32), sc.q32.view(np.int32))
@@ -200,7 +200,7 @@ def test_nan_target_takes_one_failed_step(path):
     prob, targets, _ = sc.problem()
     targets = targets.copy()
     targets[3, 5] = np.nan
-    hs = ConvergeSim(sc.model)
+    hs = HostSim(sc.model)
     q_out, err, steps, st = hs.converge(prob, sc.q32, targets, 0b01, 1e-4, 30, path=path)
     assert np.isnan(err[3]) and steps[3] == 1 and st[3] & FAILED
     np.testing.assert_array_equal(q_out[3].view(np.int32), sc.q32[3].view(np.int32))
@@ -225,7 +225,7 @@ def test_out_of_limits(safety_break):
 def test_api_errors():
     sc = helpers.ur5_scenario(4, "reachable")
     prob, targets, _ = sc.problem()
-    hs = ConvergeSim(sc.model)
+    hs = HostSim(sc.model)
     for args in ((0, 1e-3, 5), (0b100, 1e-3, 5), (0b01, -1.0, 5), (0b01, float("nan"), 5), (0b01, float("inf"), 5),
                  (0b01, 1e-3, -1)):
         with pytest.raises(RuntimeError):
@@ -262,7 +262,7 @@ def test_single_task_convergence_ur5():
     prob, parts, _ = describe_problem(model, B, [task], dt, 1e-12, [model.configuration_limit, model.velocity_limit],
                                       True)
     targets = torch.cat([x.float() for x in parts], dim=1).numpy()
-    hs = ConvergeSim(model)
+    hs = HostSim(model)
     q32 = q.astype(np.float32)
     tol = 1e-5
     q_out, err, steps, st = hs.converge(prob, q32, targets, 0b1, tol, 200)

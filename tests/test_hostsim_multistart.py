@@ -19,7 +19,7 @@ import torch
 from pink_b200 import _cabi
 from pink_b200.batched import sample_seeds
 from tests import extras, helpers
-from tests.hostsim.multistart import MultistartSim
+from tests.hostsim import HostSim
 from tests.test_hostsim_converge import FAILED, task_error
 
 
@@ -71,7 +71,7 @@ def seeds_for(sc, S, seed=0):
 def check(sc, mask, tol, max_steps, S, path=0, expect=None, qs=None):
     prob, targets, _ = sc.problem()
     qs = seeds_for(sc, S) if qs is None else qs
-    hs = MultistartSim(sc.model)
+    hs = HostSim(sc.model)
     q_out, err, seed, steps, st = hs.converge_multistart(prob, qs, targets, mask, tol, max_steps, path=path)
     if expect is not None:
         assert hs.selection.path == expect, hs.selection
@@ -113,7 +113,7 @@ def test_one_seed_equals_converge(which):
     prob, targets, _ = sc.problem()
     mask = pose_mask(prob)
     path = 1 if which == "general" else 0
-    hs = MultistartSim(sc.model)
+    hs = HostSim(sc.model)
     ref = hs.converge(prob, sc.q32, targets, mask, 1e-3, 25, path=path)
     q_out, err, seed, steps, st = hs.converge_multistart(prob, sc.q32[:, None, :], targets, mask, 1e-3, 25, path=path)
     assert hs.selection.path == which
@@ -172,7 +172,7 @@ def test_zero_steps_picks_argmin_and_duplicates_the_lowest(path):
     prob, targets, _ = sc.problem()
     qs = seeds_for(sc, 4)
     qs[:, 3] = qs[:, 1]  # seeds 1 and 3 tie
-    hs = MultistartSim(sc.model)
+    hs = HostSim(sc.model)
     q_out, err, seed, steps, st = hs.converge_multistart(prob, qs, targets, 0b01, 1e-6, 0, path=path)
     e = task_error(hs, sc.table, prob, 0b01, qs.reshape(-1, sc.table.nq), np.repeat(targets, 4, axis=0)).reshape(16, 4)
     np.testing.assert_array_equal(seed, np.argmin(e, axis=1))
@@ -189,7 +189,7 @@ def test_nan_seed_never_wins(path):
     qs = seeds_for(sc, 4)
     qs[0, 2] = np.nan  # one NaN seed in group 0
     qs[1, :] = np.nan  # group 1 all NaN
-    hs = MultistartSim(sc.model)
+    hs = HostSim(sc.model)
     q_out, err, seed, steps, st = hs.converge_multistart(prob, qs, targets, mask, 1e-3, 10, path=path)
     assert seed[0] != 2 and np.isfinite(err[0])
     assert seed[1] == 0 and np.isnan(err[1]) and steps[1] == 1 and st[1] & FAILED
@@ -203,7 +203,7 @@ def test_out_of_limits_seed_fails_while_its_group_goes_on():
     prob, targets, _ = sc.problem()
     qs = seeds_for(sc, 2)
     qs[:, 1, 0] = 10.0  # outside the limits of joint 0
-    hs = MultistartSim(sc.model)
+    hs = HostSim(sc.model)
     _, err, seed, steps, st = check(sc, 0b01, 1e-4, 20, 2, qs=qs)
     assert (seed == 0).all() and (steps > 1).any()
     assert ((st & _cabi.PK_STATUS_OUT_OF_LIMITS) == 0).all()
@@ -212,7 +212,7 @@ def test_out_of_limits_seed_fails_while_its_group_goes_on():
 def test_superset_of_converge_from_seed_zero():
     sc = helpers.ur5_scenario(32, "reachable", out_of_limits=2)
     prob, targets, _ = sc.problem()
-    hs = MultistartSim(sc.model)
+    hs = HostSim(sc.model)
     _, err1, steps1, _ = hs.converge(prob, sc.q32, targets, 0b01, 1e-4, 40)
     _, err, seed, steps, _ = hs.converge_multistart(prob, seeds_for(sc, 8), targets, 0b01, 1e-4, 40)
     solved = err1 <= 1e-4
@@ -267,7 +267,7 @@ def test_sample_seeds_continuous_and_unbounded_prismatic():
 def test_argument_errors():
     sc = helpers.ur5_scenario(4, "reachable")
     prob, targets, _ = sc.problem()
-    hs = MultistartSim(sc.model)
+    hs = HostSim(sc.model)
     qs = seeds_for(sc, 4)
     for args in ((0, 1e-3, 5), (0b100, 1e-3, 5), (0b01, -1.0, 5), (0b01, float("nan"), 5), (0b01, 1e-3, -1)):
         with pytest.raises(RuntimeError):
@@ -281,5 +281,5 @@ def test_argument_errors():
     sc = helpers.humanoid_scenario("g1_description", 2, with_com=True)
     prob, targets, _ = sc.problem()
     with pytest.raises(RuntimeError, match="at most 8"):
-        hs = MultistartSim(sc.model)
+        hs = HostSim(sc.model)
         hs.converge_multistart(prob, np.repeat(sc.q32[:, None], 16, axis=1), targets, pose_mask(prob), 1e-3, 5)
