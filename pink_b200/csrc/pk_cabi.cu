@@ -99,6 +99,20 @@ extern "C" int pk_struct_size(int which) {
 }
 extern "C" const char* pk_last_error(void) { return g_error.c_str(); }
 extern "C" int64_t pk_launch_count(void) { return g_launches.load(); }
+#ifdef PK_CHAIN_PHASE_CLOCKS
+// Copies the phase records (pk::ChainPhaseRecord, pk_math.cuh) of the warps that started since
+// the last call, at most n, to host memory `dst` and frees every slot; returns the number
+// copied, or -1 on a CUDA error.  Instrumented builds only; call with the device idle.
+extern "C" int pk_chain_phase_records(void* dst, int n, int warps_per_cta) {
+  unsigned ctas = 0u;
+  if (cudaMemcpyFromSymbol(&ctas, pk::g_chain_phase_ctas, sizeof(ctas)) != cudaSuccess) return -1;
+  n = (int)std::min<int64_t>({(int64_t)std::max(n, 0), (int64_t)pk::kChainPhaseMaxWarps, (int64_t)ctas * warps_per_cta});
+  if (n > 0 && cudaMemcpyFromSymbol(dst, pk::g_chain_phase, sizeof(pk::ChainPhaseRecord) * n) != cudaSuccess) return -1;
+  ctas = 0u;
+  if (cudaMemcpyToSymbol(pk::g_chain_phase_ctas, &ctas, sizeof(ctas)) != cudaSuccess) return -1;
+  return n;
+}
+#endif
 
 extern "C" int pk_model_create(const PkModelDesc* d, int device, PkModel** out) {
   if (!d || !out) return fail("pk_model_create: null argument");
@@ -370,6 +384,7 @@ __global__ void __launch_bounds__(128, 4)
                     const float* __restrict__ targets, float* __restrict__ v, int32_t* __restrict__ status,
                     int64_t B, int flags, int n_steps, float* __restrict__ q_out,
                     const __grid_constant__ PeerOut peers, const __grid_constant__ Trajectory T) {
+  PK_PHASE(kPhaseEntry);
   if constexpr (PDL) pdl_launch_dependents();
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   peer_gate(peers);
@@ -422,6 +437,7 @@ __global__ void __launch_bounds__(128, 4)
       for (int k = 0; k < NJ; ++k) qi[k] = used_q[k];
     }
   }
+  PK_PHASE(kPhaseWaited);
   if (v) {
     float* vrow = v + i * NJ;
     if constexpr (NJ % 2 == 0) {
@@ -474,6 +490,7 @@ __global__ void __launch_bounds__(128, 4)
   }
   if (status) status[i] = st_all;
   peer_count_kernel(peers);
+  PK_PHASE(kPhaseStored);
 }
 
 // Solve to a tolerance on chains (pk_converge_prepared): converge_chain per thread, q in

@@ -27,18 +27,15 @@ constexpr int kChainMaxFrameTasks = 2;
 PK_HD constexpr int chain_row_words(int nj, int nft) { return 12 * nft + 2 * nj; }
 
 struct ChainJoint {
-  float X[12];  // placement in the parent joint frame, row-major [R | p]
-  float ax, ay, az;
+  // X~_j: placement in the parent joint frame with every joint axis re-oriented to the local
+  // z axis (z_axis_joint_frames, pk_marshal.hpp), row-major [R | p]
+  float X[12];
   int type;  // PK_JOINT_*
-  // X.R Rot(a, q) = X.R + sin q (X.R [a]x) + (1 - cos q) (X.R (a a^T - I)): the two
-  // constant matrices, and X.R a for prismatic joints, are folded on the host
-  float M1[9], M2[9];
-  float Xa[3];
 };
 
 struct ChainFrameTask {
   int body;       // joint index the frame is fixed to (-1: world)
-  float X[12];    // frame placement in that body
+  float X[12];    // frame placement in that body's z-axis frame (z_axis_frame), or in the world
   float cost[6];  // [pos(3), ori(3)]
   float gain, lm;
   int tgt_off;
@@ -97,7 +94,8 @@ struct ChainStep {
   skip = status && P.safety_break;
   if (skip && !ERR) return status;
 
-  // ---- forward kinematics: oMi[j] = oMi[j-1] X_j exp(S_j q_j) -----------------
+  // ---- forward kinematics in z-axis joint frames: T~_j = T~_{j-1} X~_j M_z(q_j) ---------
+  // T~_j has the origin of oMi[j] and the world axis of joint j as its third column
   SE3f T = identity_se3();
   V3 pj[NJ], wj[NJ];  // world origin and world axis of every joint
   SE3f Tf[NFT > 0 ? NFT : 1], Tb[NFT > 0 ? NFT : 1];
@@ -106,23 +104,22 @@ struct ChainStep {
 #pragma unroll
   for (int j = 0; j < NJ; ++j) {
     const ChainJoint& Jn = P.joint[j];
-    const V3 axis = v3(Jn.ax, Jn.ay, Jn.az);
-    SE3f X = load_se3(Jn.X);
-    SE3f Tl;
+    const SE3f X = load_se3(Jn.X);
+    T = (j == 0) ? X : compose(T, X);  // T~_{-1} = I
     if (Jn.type == PK_JOINT_REVOLUTE) {
       float s, c;
       sincos_f(q[j], &s, &c);
-      const float t = 1.f - c;
 #pragma unroll
-      for (int k = 0; k < 9; ++k) Tl.R.m[k] = fmaf(s, Jn.M1[k], fmaf(t, Jn.M2[k], X.R.m[k]));
-      Tl.p = X.p;
+      for (int r = 0; r < 3; ++r) {  // R Rz(q): rotate the first two columns
+        const float x = T.R.m[3 * r], y = T.R.m[3 * r + 1];
+        T.R.m[3 * r] = fmaf(c, x, s * y);
+        T.R.m[3 * r + 1] = fmaf(c, y, -s * x);
+      }
     } else {
-      Tl.R = X.R;
-      Tl.p = X.p + q[j] * v3(Jn.Xa[0], Jn.Xa[1], Jn.Xa[2]);
+      T.p = T.p + q[j] * v3(T.R.m[2], T.R.m[5], T.R.m[8]);
     }
-    T = compose(T, Tl);
     pj[j] = T.p;
-    wj[j] = mul(T.R, axis);
+    wj[j] = v3(T.R.m[2], T.R.m[5], T.R.m[8]);
     // remember the placement of the joint that carries each task frame (selects only;
     // the frame offset is composed once, after the sweep)
 #pragma unroll
@@ -166,8 +163,21 @@ struct ChainStep {
       for (int k = 0; k < 3; ++k) Ttb.R.m[3 * i + k] = Tbt.R.m[3 * k + i];
     Ttb.p = -1.f * mul(Ttb.R, Tbt.p);
     L.w = -1.f * L.w;
-    M3 Am, Bm;
-    jlog6(Ttb, L, Am, Bm);
+    M3 Am, Cm;
+    jlog6_ac(Ttb, L, Am, Cm);
+    // A column of the task is -diag(cost) [Am Tf^T lin + Cm Am Tf^T ang; Am Tf^T ang]: the
+    // three 3x3 factors are formed once per task, so that a column costs 27 FMAs
+    const M3 G = mulNT(Am, Tf[t].R);
+    const M3 CG = mul(Cm, G);
+    M3 Pl, Ql, Pa;
+#pragma unroll
+    for (int i = 0; i < 3; ++i)
+#pragma unroll
+      for (int k = 0; k < 3; ++k) {
+        Pl.m[3 * i + k] = -Kt.cost[i] * G.m[3 * i + k];
+        Ql.m[3 * i + k] = -Kt.cost[i] * CG.m[3 * i + k];
+        Pa.m[3 * i + k] = -Kt.cost[3 + i] * G.m[3 * i + k];
+      }
 
     float mu = 0.f;
 #pragma unroll
@@ -180,25 +190,22 @@ struct ChainStep {
 
 #pragma unroll
     for (int j = 0; j < NJ; ++j) {
-      V3 lin, ang;
+      V3 tl, ta;
       if (P.joint[j].type == PK_JOINT_REVOLUTE) {
-        ang = wj[j];
-        lin = cross(wj[j], Tf[t].p - pj[j]);
+        const V3 lin = cross(wj[j], Tf[t].p - pj[j]);
+        tl = mul(Pl, lin) + mul(Ql, wj[j]);
+        ta = mul(Pa, wj[j]);
       } else {
-        ang = v3(0.f, 0.f, 0.f);
-        lin = wj[j];
+        tl = mul(Pl, wj[j]);
+        ta = v3(0.f, 0.f, 0.f);
       }
-      const V3 jl = mulT(Tf[t].R, lin);
-      const V3 ja = mulT(Tf[t].R, ang);
-      const V3 tl = mul(Am, jl) + mul(Bm, ja);
-      const V3 ta = mul(Am, ja);
-      const float on = (j <= Kt.body) ? -1.f : 0.f;  // joints past the frame do not move it
-      A[6 * t + 0][j] = on * Kt.cost[0] * tl.x;
-      A[6 * t + 1][j] = on * Kt.cost[1] * tl.y;
-      A[6 * t + 2][j] = on * Kt.cost[2] * tl.z;
-      A[6 * t + 3][j] = on * Kt.cost[3] * ta.x;
-      A[6 * t + 4][j] = on * Kt.cost[4] * ta.y;
-      A[6 * t + 5][j] = on * Kt.cost[5] * ta.z;
+      const float on = (j <= Kt.body) ? 1.f : 0.f;  // joints past the frame do not move it
+      A[6 * t + 0][j] = on * tl.x;
+      A[6 * t + 1][j] = on * tl.y;
+      A[6 * t + 2][j] = on * tl.z;
+      A[6 * t + 3][j] = on * ta.x;
+      A[6 * t + 4][j] = on * ta.y;
+      A[6 * t + 5][j] = on * ta.z;
     }
   }
 
@@ -265,6 +272,7 @@ PK_HD void ik_step_chain(const ChainParams<NJ>& P, const float (&q)[NJ], const f
   ChainStep<NJ, NFT> C;
   bool skip;
   int status = C.assemble(P, q, trow, skip);
+  PK_PHASE(kPhaseAssembled);
   float x[NJ];
 #pragma unroll
   for (int j = 0; j < NJ; ++j) x[j] = 0.f;

@@ -409,6 +409,7 @@ struct BoxLSQChol {
         if (lam < -4e-6f * gabs[i]) neg |= (1u << i);
       }
     }
+    PK_PHASE(kPhaseCorner);
 #ifdef PK_COUNT_ITERS
     if (act == ALL && neg == 0u) pk_count_nfree(0, -1);
 #endif
@@ -425,6 +426,7 @@ struct BoxLSQChol {
     // the KKT signs of the others with g_j + H_jF delta_F.  Anything else (a released
     // coordinate that reaches its other bound, a third release) goes to the rounds.
     if (closed_form && act == ALL && neg != 0u) {
+      PK_PHASE_FLAG(kFlagRelease1);
       // most negative multiplier
       float worst = 0.f;
       uint32_t n1 = 0u;
@@ -502,6 +504,7 @@ struct BoxLSQChol {
       if (ok) {
         // second release i2: exact minimiser over {i1, i2} from the corner, or over {i2}
         // alone when i1 sits on its opposite bound
+        PK_PHASE_FLAG(kFlagRelease2);
         float m2[N], h2[N];
 #pragma unroll
         for (int j = 0; j < N; ++j) {
@@ -815,7 +818,10 @@ struct BoxLSQChol {
     const ArrayObjective O{A, b, d, beta};
     // flags: bit 0 = closed-form first releases off (A/B), bit 1 = stop after the corner
     // stage (timing probe only: wrong results for the instances that need rounds)
-    if (corner_start(O, lo, hi, S, !(flags & 1)) && !(flags & 2)) {
+    const bool rounds = corner_start(O, lo, hi, S, !(flags & 1));
+    PK_PHASE(kPhaseClosedForm);
+    if (rounds && !(flags & 2)) {
+      PK_PHASE_FLAG(kFlagRounds);
       gram(O, S);
       bool more = true;
       for (;;) {
@@ -824,6 +830,7 @@ struct BoxLSQChol {
         if (!more) break;
       }
     }
+    PK_PHASE(kPhaseRounds);
 #pragma unroll
     for (int i = 0; i < N; ++i) x[i] = S.x[i];
     return S.status;

@@ -508,6 +508,69 @@ inline TreePlan make_tree_plan(const HostModel& m, const DevProblem& P, bool* ok
   return L;
 }
 
+// Joint frames re-oriented so that every joint axis is the local z axis.  With A_j the rotation
+// that takes e_z to the axis a_j, T~_j = oMi[j] A_j satisfies T~_j = T~_{j-1} X~_j M_z(q_j),
+// X~_j = A_{j-1}^T X_j A_j (A_{-1} = I), and a frame fixed to joint b sits at A_b^T X_f in T~_b.
+// T~_j has the origin of oMi[j] and the joint's world axis as its third column.  All folding in
+// double.  Out: Xr[9 j..] / Xp[3 j..] = rotation / translation of X~_j (row-major), A[9 j..] = A_j.
+inline void z_axis_joint_frames(const HostModel& m, int nj, float* Xr, float* Xp, double* Aall) {
+  double Aprev[9] = {1, 0, 0, 0, 1, 0, 0, 0, 1};
+  for (int j = 0; j < nj; ++j) {
+    const double a[3] = {m.axis[3 * j], m.axis[3 * j + 1], m.axis[3 * j + 2]};
+    double A[9];
+    const double c = a[2];  // e_z . a
+    if (c > 1.0 - 1e-12) {
+      const double I[9] = {1, 0, 0, 0, 1, 0, 0, 0, 1};
+      memcpy(A, I, sizeof(A));
+    } else if (c < -1.0 + 1e-12) {
+      const double Rx[9] = {1, 0, 0, 0, -1, 0, 0, 0, -1};  // half turn about x
+      memcpy(A, Rx, sizeof(A));
+    } else {
+      // Rodrigues about v = e_z x a = (-a_y, a_x, 0): A = I + [v]x + [v]x^2 / (1 + c)
+      const double vx = -a[1], vy = a[0];
+      const double k = 1.0 / (1.0 + c);
+      const double Kx[9] = {0, 0, vy, 0, 0, -vx, -vy, vx, 0};
+      for (int r = 0; r < 3; ++r)
+        for (int cc = 0; cc < 3; ++cc) {
+          double k2 = 0.0;
+          for (int t = 0; t < 3; ++t) k2 += Kx[3 * r + t] * Kx[3 * t + cc];
+          A[3 * r + cc] = (r == cc ? 1.0 : 0.0) + Kx[3 * r + cc] + k * k2;
+        }
+    }
+    memcpy(&Aall[9 * j], A, sizeof(A));
+    const float* Xj = &m.jX[12 * j];
+    // X~.R = Aprev^T X.R A, X~.p = Aprev^T X.p
+    double XA[9];
+    for (int r = 0; r < 3; ++r)
+      for (int cc = 0; cc < 3; ++cc) {
+        double s = 0.0;
+        for (int t = 0; t < 3; ++t) s += (double)Xj[4 * r + t] * A[3 * t + cc];
+        XA[3 * r + cc] = s;
+      }
+    for (int r = 0; r < 3; ++r) {
+      for (int cc = 0; cc < 3; ++cc) {
+        double s = 0.0;
+        for (int t = 0; t < 3; ++t) s += Aprev[3 * t + r] * XA[3 * t + cc];
+        Xr[9 * j + 3 * r + cc] = (float)s;
+      }
+      double sp = 0.0;
+      for (int t = 0; t < 3; ++t) sp += Aprev[3 * t + r] * (double)Xj[4 * t + 3];
+      Xp[3 * j + r] = (float)sp;
+    }
+    memcpy(Aprev, A, sizeof(A));
+  }
+}
+
+// Placement of a frame fixed to joint b in the re-oriented frame T~_b: A_b^T X_f (row-major [R | p]).
+inline void z_axis_frame(const double* A, const float* Xf, float* out) {
+  for (int r = 0; r < 3; ++r)
+    for (int cc = 0; cc < 4; ++cc) {
+      double s = 0.0;
+      for (int k = 0; k < 3; ++k) s += A[3 * k + r] * (double)Xf[4 * k + cc];
+      out[4 * r + cc] = (float)s;
+    }
+}
+
 template <int NJ>
 void make_chain_params(const HostModel& m, const DevProblem& P, ChainParams<NJ>* out, const DevExtras* X = nullptr) {
   ChainParams<NJ>& C = *out;
@@ -522,35 +585,15 @@ void make_chain_params(const HostModel& m, const DevProblem& P, ChainParams<NJ>*
       C.acc_qhi[j] = X->acc_qhi[j];
     }
   }
+  double Aall[9 * NJ];
+  float Xr[9 * NJ], Xp[3 * NJ];
+  z_axis_joint_frames(m, NJ, Xr, Xp, Aall);
   for (int j = 0; j < NJ; ++j) {
-    memcpy(C.joint[j].X, &m.jX[12 * j], sizeof(float) * 12);
-    C.joint[j].ax = m.axis[3 * j];
-    C.joint[j].ay = m.axis[3 * j + 1];
-    C.joint[j].az = m.axis[3 * j + 2];
-    C.joint[j].type = m.jtype[j];
-    {
-      // fold the constant factors of X.R Rot(a, q) in double precision
-      const float* X = &m.jX[12 * j];
-      const double a[3] = {m.axis[3 * j], m.axis[3 * j + 1], m.axis[3 * j + 2]};
-      const double Kx[9] = {0, -a[2], a[1], a[2], 0, -a[0], -a[1], a[0], 0};
-      double R[9];
-      for (int r = 0; r < 3; ++r)
-        for (int c = 0; c < 3; ++c) R[3 * r + c] = X[4 * r + c];
-      for (int r = 0; r < 3; ++r) {
-        double xa = 0.0;
-        for (int c = 0; c < 3; ++c) {
-          double m1 = 0.0, m2 = 0.0;
-          for (int k = 0; k < 3; ++k) {
-            m1 += R[3 * r + k] * Kx[3 * k + c];
-            m2 += R[3 * r + k] * (a[k] * a[c] - (k == c ? 1.0 : 0.0));
-          }
-          C.joint[j].M1[3 * r + c] = (float)m1;
-          C.joint[j].M2[3 * r + c] = (float)m2;
-          xa += R[3 * r + c] * a[c];
-        }
-        C.joint[j].Xa[r] = (float)xa;
-      }
+    for (int r = 0; r < 3; ++r) {
+      for (int c = 0; c < 3; ++c) C.joint[j].X[4 * r + c] = Xr[9 * j + 3 * r + c];
+      C.joint[j].X[4 * r + 3] = Xp[3 * j + r];
     }
+    C.joint[j].type = m.jtype[j];
     C.cfg_lo[j] = P.cfg_lo[j];
     C.cfg_hi[j] = P.cfg_hi[j];
     C.vel[j] = P.vel[j];
@@ -568,7 +611,8 @@ void make_chain_params(const HostModel& m, const DevProblem& P, ChainParams<NJ>*
     if (d.type == PK_TASK_FRAME) {
       ChainFrameTask& f = C.ft[C.n_frame_tasks++];
       f.body = d.body;
-      memcpy(f.X, &m.fX[12 * d.frame], sizeof(float) * 12);
+      if (d.body >= 0) z_axis_frame(&Aall[9 * d.body], &m.fX[12 * d.frame], f.X);
+      else memcpy(f.X, &m.fX[12 * d.frame], sizeof(float) * 12);
       memcpy(f.cost, d.cost, sizeof(float) * 6);
       f.gain = d.gain;
       f.lm = d.lm;
@@ -596,9 +640,7 @@ void make_chain_params(const HostModel& m, const DevProblem& P, ChainParams<NJ>*
 }
 
 // Parameter block of the sub-warp chain kernel (pk_coop.cuh): joint frames re-oriented so
-// that every joint axis is the local z axis.  With A_j the rotation that takes e_z to the
-// axis a_j, T~_j = oMi[j] A_j satisfies T~_j = T~_{j-1} X~_j M_z(q_j), X~_j = A_{j-1}^T X_j A_j
-// (A_{-1} = I), and a frame fixed to joint b sits at A_b^T X_f in T~_b.  All folding in double.
+// that every joint axis is the local z axis (z_axis_joint_frames).
 template <int NJ, int L>
 void make_coop_params(const HostModel& m, const DevProblem& P, CoopParams<((NJ + L - 1) / L) * L>* out,
                       const DevExtras* X = nullptr) {
@@ -610,52 +652,13 @@ void make_coop_params(const HostModel& m, const DevProblem& P, CoopParams<((NJ +
     C.acc_enabled = 1;
     C.acc_prev_off = X->acc_prev_shared ? -1 : X->acc_prev_off;
   }
-  double Aprev[9] = {1, 0, 0, 0, 1, 0, 0, 0, 1};
   std::vector<double> Aall(9 * NJ);
+  std::vector<float> Xr(9 * NJ), Xp(3 * NJ);
+  z_axis_joint_frames(m, NJ, Xr.data(), Xp.data(), Aall.data());
   for (int j = 0; j < NJ; ++j) {
-    const double a[3] = {m.axis[3 * j], m.axis[3 * j + 1], m.axis[3 * j + 2]};
-    double A[9];
-    const double c = a[2];  // e_z . a
-    if (c > 1.0 - 1e-12) {
-      const double I[9] = {1, 0, 0, 0, 1, 0, 0, 0, 1};
-      memcpy(A, I, sizeof(A));
-    } else if (c < -1.0 + 1e-12) {
-      const double Rx[9] = {1, 0, 0, 0, -1, 0, 0, 0, -1};  // half turn about x
-      memcpy(A, Rx, sizeof(A));
-    } else {
-      // Rodrigues about v = e_z x a = (-a_y, a_x, 0): A = I + [v]x + [v]x^2 / (1 + c)
-      const double vx = -a[1], vy = a[0];
-      const double k = 1.0 / (1.0 + c);
-      const double Kx[9] = {0, 0, vy, 0, 0, -vx, -vy, vx, 0};
-      for (int r = 0; r < 3; ++r)
-        for (int cc = 0; cc < 3; ++cc) {
-          double k2 = 0.0;
-          for (int t = 0; t < 3; ++t) k2 += Kx[3 * r + t] * Kx[3 * t + cc];
-          A[3 * r + cc] = (r == cc ? 1.0 : 0.0) + Kx[3 * r + cc] + k * k2;
-        }
-    }
-    memcpy(&Aall[9 * j], A, sizeof(A));
-    const float* Xj = &m.jX[12 * j];
     CoopJoint& J = C.joint[j];
-    // X~.R = Aprev^T X.R A, X~.p = Aprev^T X.p
-    double XA[9];
-    for (int r = 0; r < 3; ++r)
-      for (int cc = 0; cc < 3; ++cc) {
-        double s = 0.0;
-        for (int t = 0; t < 3; ++t) s += (double)Xj[4 * r + t] * A[3 * t + cc];
-        XA[3 * r + cc] = s;
-      }
-    for (int r = 0; r < 3; ++r) {
-      for (int cc = 0; cc < 3; ++cc) {
-        double s = 0.0;
-        for (int t = 0; t < 3; ++t) s += Aprev[3 * t + r] * XA[3 * t + cc];
-        J.Xr[3 * r + cc] = (float)s;
-      }
-      double sp = 0.0;
-      for (int t = 0; t < 3; ++t) sp += Aprev[3 * t + r] * (double)Xj[4 * t + 3];
-      J.Xp[r] = (float)sp;
-    }
-    memcpy(Aprev, A, sizeof(A));
+    memcpy(J.Xr, &Xr[9 * j], sizeof(J.Xr));
+    memcpy(J.Xp, &Xp[3 * j], sizeof(J.Xp));
     J.prismatic = (m.jtype[j] == PK_JOINT_REVOLUTE) ? 0.f : 1.f;
     if (m.jtype[j] != PK_JOINT_REVOLUTE) C.any_prismatic = 1;
     J.cfg_lo = P.cfg_lo[j];
@@ -688,13 +691,7 @@ void make_coop_params(const HostModel& m, const DevProblem& P, CoopParams<((NJ +
       f.body = d.body;
       const float* Xf = &m.fX[12 * d.frame];
       if (d.body >= 0) {
-        const double* A = &Aall[9 * d.body];
-        for (int r = 0; r < 3; ++r)
-          for (int cc = 0; cc < 4; ++cc) {
-            double s = 0.0;
-            for (int k = 0; k < 3; ++k) s += A[3 * k + r] * (double)Xf[4 * k + cc];
-            f.X[4 * r + cc] = (float)s;
-          }
+        z_axis_frame(&Aall[9 * d.body], Xf, f.X);
       } else {
         memcpy(f.X, Xf, sizeof(float) * 12);
       }

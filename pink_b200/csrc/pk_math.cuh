@@ -83,6 +83,15 @@ PK_HD M3 mulTN(const M3& A, const M3& B) {  // A^T B
       C.m[3 * i + j] = fmaf(A.m[i], B.m[j], fmaf(A.m[3 + i], B.m[3 + j], A.m[6 + i] * B.m[6 + j]));
   return C;
 }
+PK_HD M3 mulNT(const M3& A, const M3& B) {  // A B^T
+  M3 C;
+#pragma unroll
+  for (int i = 0; i < 3; ++i)
+#pragma unroll
+    for (int j = 0; j < 3; ++j)
+      C.m[3 * i + j] = fmaf(A.m[3 * i], B.m[3 * j], fmaf(A.m[3 * i + 1], B.m[3 * j + 1], A.m[3 * i + 2] * B.m[3 * j + 2]));
+  return C;
+}
 PK_HD M3 identity3() {
   M3 I;
 #pragma unroll
@@ -290,7 +299,14 @@ PK_HD void log6(const SE3f& T, const Log3& L, float e[6]) {
 
 // Jlog6(T) = [[A, B], [0, A]], A = a w w^T + (1 - theta^2 a) I + 1/2 [w]x, B = C A,
 // C = v3 w^T + a w p^T + a (w.p) I + 1/2 [p]x, v3 = adot (w.p) w - (theta^2 adot + 2 a) p.
+PK_HD void jlog6_ac(const SE3f& T, const Log3& L, M3& A, M3& C);
 PK_HD void jlog6(const SE3f& T, const Log3& L, M3& A, M3& B) {
+  M3 C;
+  jlog6_ac(T, L, A, C);
+  B = mul(C, A);
+}
+// The factors A and C of Jlog6 (B = C A), for callers that fold C into their own products.
+PK_HD void jlog6_ac(const SE3f& T, const Log3& L, M3& A, M3& C) {
   const V3 w = L.w, p = T.p;
   const float x = L.theta * L.theta;
   const float d = fmaf(-x, L.a, 1.f);
@@ -306,7 +322,6 @@ PK_HD void jlog6(const SE3f& T, const Log3& L, M3& A, M3& B) {
   const float wp = dot(w, p);
   const V3 v3_ = (L.adot * wp) * w - fmaf(x, L.adot, 2.f * L.a) * p;
   const float di = L.a * wp;
-  M3 C;
   C.m[0] = fmaf(v3_.x, w.x, fmaf(L.a * w.x, p.x, di));
   C.m[1] = fmaf(v3_.x, w.y, fmaf(L.a * w.x, p.y, -0.5f * p.z));
   C.m[2] = fmaf(v3_.x, w.z, fmaf(L.a * w.x, p.z, 0.5f * p.y));
@@ -316,7 +331,6 @@ PK_HD void jlog6(const SE3f& T, const Log3& L, M3& A, M3& B) {
   C.m[6] = fmaf(v3_.z, w.x, fmaf(L.a * w.z, p.x, -0.5f * p.y));
   C.m[7] = fmaf(v3_.z, w.y, fmaf(L.a * w.z, p.y, 0.5f * p.x));
   C.m[8] = fmaf(v3_.z, w.z, fmaf(L.a * w.z, p.z, di));
-  B = mul(C, A);
 }
 
 // q (+) v dt of one instance (Configuration.integrate, pink/configuration.py:273-283):
@@ -389,6 +403,81 @@ PK_HD void record_rows(const Trajectory& T, int s, int64_t B, int64_t i, int nq,
 PK_HD bool step_failed(int st_all, int safety_break) {
   return (st_all & (PK_STATUS_NO_SOLUTION | PK_STATUS_NOT_POSDEF)) || ((st_all & PK_STATUS_OUT_OF_LIMITS) && safety_break);
 }
+
+// Phase clocks of the chain kernel (compile-time switch PK_CHAIN_PHASE_CLOCKS, off in the
+// product build, where PK_PHASE / PK_PHASE_FLAG expand to nothing).  Every warp keeps one
+// record: %globaltimer (ns) and clock64 at each phase boundary, the largest value over its
+// lanes (lanes that leave a stage early pass the next mark first), the SM it ran on and the
+// stages at least one of its lanes entered.  CTAs take consecutive record slots in the order
+// they start, so the records of consecutive launches (which overlap under PDL) never share a
+// slot and come out grouped by launch.  Read back and reset by pk_chain_phase_records
+// (scripts/chain_phases.py).
+enum ChainPhase {
+  kPhaseEntry = 0,     // kernel entry
+  kPhaseAssembled,     // after ChainStep::assemble (limit check, FK, task rows, box)
+  kPhaseCorner,        // after the corner test of BoxLSQChol::corner_start
+  kPhaseClosedForm,    // after the closed-form releases (corner_start returned)
+  kPhaseRounds,        // after the Cholesky rounds and polish
+  kPhaseWaited,        // after griddepcontrol.wait and the re-read of the inputs
+  kPhaseStored,        // after the last store
+  kPhaseCount
+};
+enum ChainPhaseFlag { kFlagRelease1 = 1, kFlagRelease2 = 2, kFlagRounds = 4 };
+struct ChainPhaseRecord {
+  unsigned long long ns[kPhaseCount];
+  unsigned long long clk[kPhaseCount];
+  unsigned smid, flags;
+};
+constexpr int kChainPhaseMaxWarps = 65536;
+#if defined(PK_CHAIN_PHASE_CLOCKS) && defined(__CUDACC__)
+__device__ ChainPhaseRecord g_chain_phase[kChainPhaseMaxWarps];
+__device__ unsigned g_chain_phase_ctas;  // CTAs that took a slot since the last read
+#endif
+#if defined(PK_CHAIN_PHASE_CLOCKS) && defined(__CUDA_ARCH__)
+__device__ __forceinline__ unsigned& chain_phase_cta() {
+  __shared__ unsigned slot;
+  return slot;
+}
+__device__ __forceinline__ ChainPhaseRecord* chain_phase_record() {
+  const unsigned w = chain_phase_cta() * ((blockDim.x + 31) / 32) + threadIdx.x / 32;
+  return w < kChainPhaseMaxWarps ? &g_chain_phase[w] : nullptr;
+}
+// leader of the lanes active here
+__device__ __forceinline__ bool chain_phase_leader() { return (threadIdx.x & 31) == (unsigned)(__ffs(__activemask()) - 1); }
+__device__ __forceinline__ void chain_phase_mark(int k) {
+  if (k == kPhaseEntry) {  // every thread of the CTA, before any returns
+    if (threadIdx.x == 0) chain_phase_cta() = atomicAdd(&g_chain_phase_ctas, 1u);
+    __syncthreads();
+  }
+  ChainPhaseRecord* r = chain_phase_record();
+  if (!r || !chain_phase_leader()) return;
+  unsigned long long ns, clk;
+  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(ns));
+  clk = clock64();
+  if (k == kPhaseEntry) {
+    unsigned sm;
+    asm volatile("mov.u32 %0, %%smid;" : "=r"(sm));
+    for (int j = 1; j < kPhaseCount; ++j) r->ns[j] = r->clk[j] = 0ull;
+    r->ns[0] = ns;
+    r->clk[0] = clk;
+    r->smid = sm;
+    r->flags = 0u;
+    __threadfence_block();
+  } else {
+    atomicMax(&r->ns[k], ns);
+    atomicMax(&r->clk[k], clk);
+  }
+}
+__device__ __forceinline__ void chain_phase_flag(unsigned f) {
+  ChainPhaseRecord* r = chain_phase_record();
+  if (r && chain_phase_leader()) atomicOr(&r->flags, f);
+}
+#define PK_PHASE(k) ::pk::chain_phase_mark(::pk::k)
+#define PK_PHASE_FLAG(f) ::pk::chain_phase_flag(::pk::f)
+#else
+#define PK_PHASE(k) ((void)0)
+#define PK_PHASE_FLAG(f) ((void)0)
+#endif
 
 // max(m, n) that keeps a NaN: a NaN task error makes the whole error NaN (never <= tol).
 PK_HD float err_max(float m, float n) { return (n > m || n != n) ? n : m; }
