@@ -493,10 +493,9 @@ __global__ void __launch_bounds__(128, 4)
   PK_PHASE(kPhaseStored);
 }
 
-// Solve to a tolerance on chains (pk_converge_prepared): converge_chain per thread, q in
-// registers.  A plain launch: no PDL, no peer epilogue, no records.  q_out may alias q (each
-// thread reads its row before it writes it).  emask: the task mask in chain slots
-// (chain_task_mask).
+// Solve to a tolerance on chains (pk_converge_prepared): converge_chain_instance per thread, q in
+// registers.  A plain launch: no PDL, no peer epilogue, no records.  emask: the task mask in chain
+// slots (chain_task_mask).
 template <int NJ, int NFT>
 __global__ void __launch_bounds__(128, 4)
     ik_chain_converge_kernel(const __grid_constant__ ChainParams<NJ> P, const float* q,
@@ -505,17 +504,7 @@ __global__ void __launch_bounds__(128, 4)
                              int32_t* __restrict__ status, int64_t B) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= B) return;
-  float qi[NJ];
-#pragma unroll
-  for (int k = 0; k < NJ; ++k) qi[k] = q[i * NJ + k];
-  float e;
-  int n, st;
-  converge_chain<NJ, NFT>(P, qi, targets + i * (int64_t)P.target_stride, emask, tol, max_steps, e, n, st);
-#pragma unroll
-  for (int k = 0; k < NJ; ++k) q_out[i * NJ + k] = qi[k];
-  if (err) err[i] = e;
-  if (steps) steps[i] = n;
-  if (status) status[i] = st;
+  converge_chain_instance<NJ, NFT>(P, q, targets, emask, tol, max_steps, q_out, err, steps, status, i);
 }
 
 // General path: one instance per thread, per-thread arrays in local memory.
@@ -529,8 +518,7 @@ __global__ void __launch_bounds__(64) ik_generic_kernel(const DevModel M, const 
   G.step(M, P, A.q + i * M.nq, A.targets ? A.targets + i * (int64_t)P.target_stride : nullptr, out);
 }
 
-// Trajectory rollout of the general path in one launch: rollout_generic per thread on the
-// instance's q_out row in place.
+// Trajectory rollout of the general path in one launch: rollout_generic_instance per thread.
 template <int NJMAX, int NVMAX>
 __global__ void __launch_bounds__(64)
     ik_generic_rollout_kernel(const DevModel M, const __grid_constant__ DevProblem P, const float* q,
@@ -538,16 +526,11 @@ __global__ void __launch_bounds__(64)
                               int32_t* __restrict__ status, int64_t B, const __grid_constant__ Trajectory T) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= B) return;
-  const int nq = M.nq;
-  float* qrow = q_out + i * nq;
-  for (int k = 0; k < nq; ++k) qrow[k] = q[i * nq + k];
   Generic<NJMAX, NVMAX> G;
-  const int st_all = rollout_generic(G, M, P, qrow, v + i * M.nv, targets, n_steps, T, B, i);
-  if (status) status[i] = st_all;
+  rollout_generic_instance(G, M, P, q, targets, n_steps, q_out, v, status, T, B, i);
 }
 
-// Solve to a tolerance on the general path (pk_converge_prepared): converge_generic per thread
-// on the instance's q_out row in place; v in local memory.
+// Solve to a tolerance on the general path (pk_converge_prepared): converge_generic_instance per thread.
 template <int NJMAX, int NVMAX>
 __global__ void __launch_bounds__(64)
     ik_generic_converge_kernel(const DevModel M, const __grid_constant__ DevProblem P, const float* q,
@@ -556,18 +539,8 @@ __global__ void __launch_bounds__(64)
                                int64_t B) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= B) return;
-  const int nq = M.nq;
-  float* qrow = q_out + i * nq;
-  for (int k = 0; k < nq; ++k) qrow[k] = q[i * nq + k];
-  float v[NVMAX];
   Generic<NJMAX, NVMAX> G;
-  float e;
-  int n, st;
-  converge_generic(G, M, P, qrow, targets ? targets + i * (int64_t)P.target_stride : nullptr, v, mask, tol, max_steps,
-                   e, n, st);
-  if (err) err[i] = e;
-  if (steps) steps[i] = n;
-  if (status) status[i] = st;
+  converge_generic_instance(G, M, P, q, targets, mask, tol, max_steps, q_out, err, steps, status, i);
 }
 
 // Tree kernel: one instance per warp, per-instance state in the warp's slice of
@@ -586,56 +559,38 @@ __global__ void __launch_bounds__(32 * kTreeWarpsPerBlock, PK_TREE_MIN_BLOCKS)
   const int warp = threadIdx.x >> 5;
   const int64_t i = (int64_t)blockIdx.x * kTreeWarpsPerBlock + warp;
   if (i >= B) return;
-  float* W = tree_smem + (size_t)warp * L.words;
-  TreeStep::run(M, P, L, q + i * L.nq, targets ? targets + i * (int64_t)L.stride : nullptr, W, v + i * L.nv,
-                status ? status + i : nullptr);
+  TreeStep::solve_instance(M, P, L, q, targets, tree_smem + (size_t)warp * L.words, v, status, i);
 }
 
-// Closed-loop rollout of the tree kernel in ONE launch: TreeStep::rollout per warp on the
-// instance's q_out row in place, the q / v rows re-read by the warp that wrote them (they stay in
-// L1 / L2; the per-step launch pair and its two full passes over HBM are gone).
+// Closed-loop rollout of the tree kernel in ONE launch: TreeStep::rollout_instance per warp, the q / v
+// rows re-read by the warp that wrote them (they stay in L1 / L2; no per-step launch pair and its two
+// full passes over HBM).
 __global__ void __launch_bounds__(32 * kTreeWarpsPerBlock)
     ik_tree_rollout_kernel(const DevModel M, const __grid_constant__ DevProblem P, const __grid_constant__ TreePlan L,
                            const float* __restrict__ q, const float* __restrict__ targets, int n_steps,
                            float* __restrict__ q_out, float* __restrict__ v, int32_t* __restrict__ status, int64_t B,
                            const __grid_constant__ Trajectory T) {
   extern __shared__ __align__(16) float tree_smem[];
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int warp = threadIdx.x >> 5;
   const int64_t i = (int64_t)blockIdx.x * kTreeWarpsPerBlock + warp;
   if (i >= B) return;
-  float* W = tree_smem + (size_t)warp * L.words;
-  float* qrow = q_out + i * L.nq;
-  for (int k = lane; k < L.nq; k += 32) qrow[k] = q[i * L.nq + k];
-  __syncwarp();
-  const int st_all = TreeStep::rollout(M, P, L, qrow, targets, W, v + i * L.nv, n_steps, T, B, i);
-  if (status && lane == 0) status[i] = st_all;
+  TreeStep::rollout_instance(M, P, L, q, targets, n_steps, q_out, tree_smem + (size_t)warp * L.words, v, status, T, B,
+                             i);
 }
 
-// Solve to a tolerance on joint trees (pk_converge_prepared): TreeStep::converge per warp on
-// the instance's q_out row in place; the step's v at word o_v of the warp's workspace (the
-// plan's words include it).  The warp leaves its loop as soon as its instance stops.
+// Solve to a tolerance on joint trees (pk_converge_prepared): TreeStep::converge_instance per warp,
+// L and o_v from converge_tree_layout.  The warp leaves its loop as soon as its instance stops.
 __global__ void __launch_bounds__(32 * kTreeWarpsPerBlock)
     ik_tree_converge_kernel(const DevModel M, const __grid_constant__ DevProblem P, const __grid_constant__ TreePlan L,
                             int o_v, const float* q, const float* __restrict__ targets, unsigned mask, float tol,
                             int max_steps, float* q_out, float* __restrict__ err, int32_t* __restrict__ steps,
                             int32_t* __restrict__ status, int64_t B) {
   extern __shared__ __align__(16) float tree_smem[];
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int warp = threadIdx.x >> 5;
   const int64_t i = (int64_t)blockIdx.x * kTreeWarpsPerBlock + warp;
   if (i >= B) return;
-  float* W = tree_smem + (size_t)warp * L.words;
-  float* qrow = q_out + i * L.nq;
-  for (int k = lane; k < L.nq; k += 32) qrow[k] = q[i * L.nq + k];
-  __syncwarp();
-  float e;
-  int n, st;
-  TreeStep::converge(M, P, L, qrow, targets ? targets + i * (int64_t)L.stride : nullptr, W, W + o_v, mask, tol,
-                     max_steps, e, n, st);
-  if (lane == 0) {
-    if (err) err[i] = e;
-    if (steps) steps[i] = n;
-    if (status) status[i] = st;
-  }
+  TreeStep::converge_instance(M, P, L, o_v, q, targets, mask, tol, max_steps, q_out, tree_smem + (size_t)warp * L.words,
+                              err, steps, status, i);
 }
 
 // q (+) v dt
@@ -721,6 +676,13 @@ int launched() {
 const pk::PeerOut kNoPeers{};
 const pk::Trajectory kNoTrajectory{};
 
+// A kernel with one thread per row: `rows` threads in blocks of `block`.
+template <class... Params, class... Args>
+int launch_rows(void (*kernel)(Params...), int64_t rows, int block, cudaStream_t stream, const Args&... args) {
+  kernel<<<(unsigned)((rows + block - 1) / block), block, 0, stream>>>(args...);
+  return launched();
+}
+
 // a call the PDL instantiation of the chain kernel cannot run: per-step targets rows or records
 bool per_step(const pk::Trajectory& T) { return T.target_step != 0 || T.q || T.v || T.status; }
 
@@ -762,25 +724,9 @@ int launch_chain(const pk::ChainParams<NJ>& C, bool pdl_row_fits, const float* q
 // size_class: pk::generic_size_class of the model
 int launch_generic(const PkModel* m, int size_class, const pk::DevProblem& P, const pk::GenericArgs& A, int64_t B,
                    cudaStream_t stream) {
-  const int block = 64;
-  const int64_t grid = (B + block - 1) / block;
-  pk::with_generic(size_class, [&](auto nj, auto nv) {
-    pk::ik_generic_kernel<decltype(nj)::value, decltype(nv)::value><<<(unsigned)grid, block, 0, stream>>>(m->dev, P, A, B);
+  return pk::with_generic(size_class, [&](auto nj, auto nv) {
+    return launch_rows(pk::ik_generic_kernel<decltype(nj)::value, decltype(nv)::value>, B, 64, stream, m->dev, P, A, B);
   });
-  return launched();
-}
-
-// The general path's trajectory rollout: one launch of ik_generic_rollout_kernel
-int launch_generic_rollout(const PkModel* m, int size_class, const pk::DevProblem& P, const float* q,
-                           const float* targets, int n_steps, float* q_out, float* v, int32_t* status, int64_t B,
-                           cudaStream_t stream, const pk::Trajectory& traj) {
-  const int block = 64;
-  const int64_t grid = (B + block - 1) / block;
-  pk::with_generic(size_class, [&](auto nj, auto nv) {
-    pk::ik_generic_rollout_kernel<decltype(nj)::value, decltype(nv)::value>
-        <<<(unsigned)grid, block, 0, stream>>>(m->dev, P, q, targets, n_steps, q_out, v, status, B, traj);
-  });
-  return launched();
 }
 
 // Dynamic shared memory a kernel has been granted, per device ordinal: the opt-in is per device,
@@ -835,6 +781,20 @@ struct PkProblem {
   alignas(16) unsigned char chain_params[sizeof(pk::ChainParams<7>)];
   // parameter block of the sub-warp chain kernel's variant sel.lanes (the padding joints depend on it)
   alignas(16) unsigned char coop_params[sizeof(pk::CoopParams<8>)];
+
+  // the parameter blocks, typed: ik_chain_kernel<NJ, *>'s and ik_coop_kernel<NJ, NFT, L>'s
+  template <int NJ>
+  pk::ChainParams<NJ>& chain() {
+    static_assert(sizeof(pk::ChainParams<NJ>) <= sizeof(chain_params), "parameter block too small");
+    return *reinterpret_cast<pk::ChainParams<NJ>*>(chain_params);
+  }
+  template <int NJ, int NFT, int L, class Params = pk::CoopParams<pk::CoopStep<NJ, NFT, L>::NJP>>
+  Params& coop() {
+    static_assert(sizeof(Params) <= sizeof(coop_params), "parameter block too small");
+    return *reinterpret_cast<Params*>(coop_params);
+  }
+  template <int NJ> const auto& chain() const { return const_cast<PkProblem*>(this)->chain<NJ>(); }
+  template <int NJ, int NFT, int L> const auto& coop() const { return const_cast<PkProblem*>(this)->coop<NJ, NFT, L>(); }
 };
 
 namespace {
@@ -887,18 +847,13 @@ int prepare_problem(const PkModel* m, const PkProblemDesc* desc, PkProblem* pr, 
   const pk::Selection& s = pr->sel = pk::select_kernel(m->hm, pr->P, hx, opts);
   if (s.path != pk::kPathChain) return 0;
   const pk::DevExtras* X = hx.present ? &hx.X : nullptr;
-  pk::with_nj(s.nj, [&](auto nj) {
-    constexpr int NJ = decltype(nj)::value;
-    static_assert(sizeof(pk::ChainParams<NJ>) <= sizeof(pr->chain_params), "parameter block too small");
-    pk::make_chain_params<NJ>(m->hm, pr->P, reinterpret_cast<pk::ChainParams<NJ>*>(pr->chain_params), X);
+  pk::with_chain(s, [&](auto nj, auto nft) {
+    constexpr int NJ = decltype(nj)::value, NFT = decltype(nft)::value;
+    pk::make_chain_params<NJ>(m->hm, pr->P, &pr->chain<NJ>(), X);
     if (!s.lanes) return;
-    pk::with_nft(s.nft, [&](auto nft) {
-      pk::with_lanes<NJ, decltype(nft)::value>(s.lanes, [&](auto lanes) {
-        constexpr int L = decltype(lanes)::value;
-        using Params = pk::CoopParams<pk::CoopStep<NJ, decltype(nft)::value, L>::NJP>;
-        static_assert(sizeof(Params) <= sizeof(pr->coop_params), "parameter block too small");
-        pk::make_coop_params<NJ, L>(m->hm, pr->P, reinterpret_cast<Params*>(pr->coop_params), X);
-      });
+    pk::with_lanes<NJ, NFT>(s.lanes, [&](auto lanes) {
+      constexpr int L = decltype(lanes)::value;
+      pk::make_coop_params<NJ, L>(m->hm, pr->P, &pr->coop<NJ, NFT, L>(), X);
     });
   });
   return 0;
@@ -910,23 +865,17 @@ int prepare_problem(const PkModel* m, const PkProblemDesc* desc, PkProblem* pr, 
 int launch_chain_prepared(const PkProblem& pr, const float* q, const float* targets, float* v, int32_t* status,
                           int64_t B, cudaStream_t stream, int n_steps, float* q_out, const pk::PeerOut* peers,
                           const pk::Trajectory& traj = kNoTrajectory) {
-  return pk::with_nj(pr.sel.nj, [&](auto nj) {
-    constexpr int NJ = decltype(nj)::value;
-    return pk::with_nft(pr.sel.nft, [&](auto nft) {
-      constexpr int NFT = decltype(nft)::value;
-      if (pr.sel.lanes && !peers) {
-        return pk::with_lanes<NJ, NFT>(pr.sel.lanes, [&](auto lanes) {
-          constexpr int L = decltype(lanes)::value;
-          const auto& C = *reinterpret_cast<const pk::CoopParams<pk::CoopStep<NJ, NFT, L>::NJP>*>(pr.coop_params);
-          const int64_t grid = (B * L + pk::kCoopThreads - 1) / pk::kCoopThreads;
-          pk::ik_coop_kernel<NJ, NFT, L>
-              <<<(unsigned)grid, pk::kCoopThreads, 0, stream>>>(C, q, targets, v, status, B, n_steps, q_out, traj);
-          return launched();
-        });
-      }
-      return launch_chain<NJ, NFT>(*reinterpret_cast<const pk::ChainParams<NJ>*>(pr.chain_params), pr.sel.pdl_row_fits,
-                                   q, targets, v, status, B, stream, n_steps, q_out, peers ? *peers : kNoPeers, traj);
-    });
+  return pk::with_chain(pr.sel, [&](auto nj, auto nft) {
+    constexpr int NJ = decltype(nj)::value, NFT = decltype(nft)::value;
+    if (pr.sel.lanes && !peers) {
+      return pk::with_lanes<NJ, NFT>(pr.sel.lanes, [&](auto lanes) {
+        constexpr int L = decltype(lanes)::value;
+        return launch_rows(pk::ik_coop_kernel<NJ, NFT, L>, B * L, pk::kCoopThreads, stream, pr.coop<NJ, NFT, L>(), q,
+                           targets, v, status, B, n_steps, q_out, traj);
+      });
+    }
+    return launch_chain<NJ, NFT>(pr.chain<NJ>(), pr.sel.pdl_row_fits, q, targets, v, status, B, stream, n_steps, q_out,
+                                 peers ? *peers : kNoPeers, traj);
   });
 }
 
@@ -954,6 +903,18 @@ int check_common(const PkModel* m, const void* q, int64_t B) {
   return 0;
 }
 
+// The argument checks of the *_prepared entries, in this order: check_common, the problem, the
+// entry's own checks `more()` (nonzero: failed), the targets.
+template <class More>
+int check_prepared(const PkModel* m, const PkProblem* pr, const void* q, const void* targets, int64_t B, More more) {
+  if (check_common(m, q, B)) return 1;
+  if (!pr) return fail("null problem");
+  if (more()) return 1;
+  if (B > 0 && pr->P.target_stride > 0 && !targets) return fail("null targets");
+  return 0;
+}
+int no_more_checks() { return 0; }
+
 }  // namespace
 
 // --------------------------------------------------------------------------------------
@@ -978,20 +939,14 @@ static int solve_host_impl(PkModel* m, const PkProblem& pr, const float* q_host,
 
 extern "C" int pk_solve_ik_prepared(const PkModel* m, const PkProblem* pr, const float* q, const float* targets,
                                     float* v, int32_t* status, int64_t B, void* stream) {
-  if (check_common(m, q, B)) return 1;
-  if (!pr) return fail("null problem");
-  if (B > 0 && !v) return fail("null v");
-  if (B > 0 && pr->P.target_stride > 0 && !targets) return fail("null targets");
+  if (check_prepared(m, pr, q, targets, B, [&] { return B > 0 && !v ? fail("null v") : 0; })) return 1;
   return solve_device(m, *pr, q, targets, v, status, B, (cudaStream_t)stream);
 }
 
 extern "C" int pk_solve_ik_prepared_host(PkModel* m, const PkProblem* pr, const float* q_host,
                                          const float* targets_host, float* v_host, int32_t* status_host, int64_t B,
                                          void* stream) {
-  if (check_common(m, q_host, B)) return 1;
-  if (!pr) return fail("null problem");
-  if (B > 0 && !v_host) return fail("null v");
-  if (B > 0 && pr->P.target_stride > 0 && !targets_host) return fail("null targets");
+  if (check_prepared(m, pr, q_host, targets_host, B, [&] { return B > 0 && !v_host ? fail("null v") : 0; })) return 1;
   return solve_host_impl(m, *pr, q_host, targets_host, v_host, status_host, B, (cudaStream_t)stream);
 }
 
@@ -1067,9 +1022,7 @@ extern "C" int pk_solve_ik_prepared_gather(const PkModel* m, const PkProblem* pr
                                            float* v, int32_t* status, int64_t B, void* const* peer_v,
                                            int32_t n_peers, int64_t row_offset, void* const* peer_flags,
                                            int32_t rank, int32_t n_buffers, void* stream_) {
-  if (check_common(m, q, B)) return 1;
-  if (!pr) return fail("null problem");
-  if (B > 0 && pr->P.target_stride > 0 && !targets) return fail("null targets");
+  if (check_prepared(m, pr, q, targets, B, no_more_checks)) return 1;
   if (B == 0) return 0;
   cudaStream_t stream = (cudaStream_t)stream_;
   pk::PeerOut po;
@@ -1106,19 +1059,19 @@ extern "C" int pk_peer_sync(int device, void* const* peer_flags, int32_t n_peers
 extern "C" int pk_rollout_prepared(const PkModel* m, const PkProblem* pr, const float* q, const float* targets,
                                    int32_t n_steps, float* q_out, float* v, int32_t* status, int64_t B,
                                    void* stream_) {
-  if (check_common(m, q, B)) return 1;
-  if (!pr) return fail("null problem");
-  if (n_steps < 1) return fail("n_steps must be >= 1");
-  if (B > 0 && (!v || !q_out)) return fail("null v or q_out");
-  if (B > 0 && pr->P.target_stride > 0 && !targets) return fail("null targets");
+  if (check_prepared(m, pr, q, targets, B, [&] {
+        if (n_steps < 1) return fail("n_steps must be >= 1");
+        return B > 0 && (!v || !q_out) ? fail("null v or q_out") : 0;
+      }))
+    return 1;
   if (B == 0) return 0;
   cudaStream_t stream = (cudaStream_t)stream_;
-  if (pr->sel.path == pk::kPathChain)
-    return launch_chain_prepared(*pr, q, targets, v, status, B, stream, n_steps, q_out, nullptr);
-  if (pr->sel.path == pk::kPathTree)  // joint trees: the whole loop in one launch of the warp kernel
-    return launch_tree_warps(pk::ik_tree_rollout_kernel, g_tree_rollout_smem, m, pr->sel.plan, B, stream, m->dev,
-                             pr->P, pr->sel.plan, q, targets, n_steps, q_out, v, status, B, kNoTrajectory);
-  // other models: the same closed loop as separate launches (solve, then integrate in place)
+  // chains and joint trees: the whole loop in one launch, the trajectory kernels with fixed rows
+  // and no records
+  if (pr->sel.path != pk::kPathGeneral)
+    return pk_rollout_trajectory_prepared(m, pr, q, targets, 0, n_steps, q_out, v, status, nullptr, nullptr, nullptr, B,
+                                          stream_);
+  // the general path: the same closed loop as separate launches (solve, then integrate in place)
   if (q_out != q) PK_CUDA(cudaMemcpyAsync(q_out, q, sizeof(float) * B * m->nq, cudaMemcpyDeviceToDevice, stream));
   for (int s = 0; s < n_steps; ++s) {
     if (solve_device(m, *pr, q_out, targets, v, status, B, stream)) return 1;
@@ -1131,12 +1084,12 @@ extern "C" int pk_rollout_trajectory_prepared(const PkModel* m, const PkProblem*
                                               const float* targets, int64_t target_step, int32_t n_steps,
                                               float* q_out, float* v, int32_t* status, float* q_traj, float* v_traj,
                                               int32_t* status_traj, int64_t B, void* stream_) {
-  if (check_common(m, q, B)) return 1;
-  if (!pr) return fail("null problem");
-  if (n_steps < 1) return fail("n_steps must be >= 1");
-  if (target_step < 0) return fail("negative target_step");
-  if (B > 0 && (!v || !q_out)) return fail("null v or q_out");
-  if (B > 0 && pr->P.target_stride > 0 && !targets) return fail("null targets");
+  if (check_prepared(m, pr, q, targets, B, [&] {
+        if (n_steps < 1) return fail("n_steps must be >= 1");
+        if (target_step < 0) return fail("negative target_step");
+        return B > 0 && (!v || !q_out) ? fail("null v or q_out") : 0;
+      }))
+    return 1;
   if (B == 0) return 0;
   cudaStream_t stream = (cudaStream_t)stream_;
   const pk::Trajectory traj{target_step, q_traj, v_traj, status_traj};
@@ -1145,70 +1098,60 @@ extern "C" int pk_rollout_trajectory_prepared(const PkModel* m, const PkProblem*
   if (pr->sel.path == pk::kPathTree)
     return launch_tree_warps(pk::ik_tree_rollout_kernel, g_tree_rollout_smem, m, pr->sel.plan, B, stream, m->dev,
                              pr->P, pr->sel.plan, q, targets, n_steps, q_out, v, status, B, traj);
-  return launch_generic_rollout(m, pr->sel.generic_class, pr->P, q, targets, n_steps, q_out, v, status, B, stream,
-                                traj);
+  return pk::with_generic(pr->sel.generic_class, [&](auto nj, auto nv) {
+    return launch_rows(pk::ik_generic_rollout_kernel<decltype(nj)::value, decltype(nv)::value>, B, 64, stream, m->dev,
+                       pr->P, q, targets, n_steps, q_out, v, status, B, traj);
+  });
 }
 
 extern "C" int pk_converge_prepared(const PkModel* m, const PkProblem* pr, const float* q, const float* targets,
                                     uint32_t task_mask, float tol, int32_t max_steps, float* q_out, float* err,
                                     int32_t* steps, int32_t* status, int64_t B, void* stream_) {
-  if (check_common(m, q, B)) return 1;
-  if (!pr) return fail("null problem");
-  const std::string aerr = pk::check_converge_args(pr->P, task_mask, tol, max_steps);
-  if (!aerr.empty()) return fail(aerr);
-  if (B > 0 && !q_out) return fail("null q_out");
-  if (B > 0 && pr->P.target_stride > 0 && !targets) return fail("null targets");
+  if (check_prepared(m, pr, q, targets, B, [&] {
+        const std::string aerr = pk::check_converge_args(pr->P, task_mask, tol, max_steps);
+        if (!aerr.empty()) return fail(aerr);
+        return B > 0 && !q_out ? fail("null q_out") : 0;
+      }))
+    return 1;
   if (B == 0) return 0;
   cudaStream_t stream = (cudaStream_t)stream_;
   const pk::Selection& sel = pr->sel;
   if (sel.path == pk::kPathChain) {
     // always the thread-per-instance kernel: PK_CHAIN_LANES selects only the solve entries' variant
     const unsigned emask = pk::chain_task_mask(pr->P, task_mask, sel.nft);
-    const int block = 128;
-    const int64_t grid = (B + block - 1) / block;
-    pk::with_nj(sel.nj, [&](auto nj) {
+    return pk::with_chain(sel, [&](auto nj, auto nft) {
       constexpr int NJ = decltype(nj)::value;
-      pk::with_nft(sel.nft, [&](auto nft) {
-        pk::ik_chain_converge_kernel<NJ, decltype(nft)::value><<<(unsigned)grid, block, 0, stream>>>(
-            *reinterpret_cast<const pk::ChainParams<NJ>*>(pr->chain_params), q, targets, emask, tol, max_steps, q_out,
-            err, steps, status, B);
-      });
+      return launch_rows(pk::ik_chain_converge_kernel<NJ, decltype(nft)::value>, B, 128, stream, pr->chain<NJ>(), q,
+                         targets, emask, tol, (int)max_steps, q_out, err, steps, status, B);
     });
-    return launched();
   }
   if (sel.path == pk::kPathTree) {
-    // the step's v lives in the warp's workspace, after the plan's words (kept 4-word aligned)
-    pk::TreePlan plan = sel.plan;
-    const int o_v = plan.words;
-    plan.words += (plan.nv + 3) & ~3;
-    return launch_tree_warps(pk::ik_tree_converge_kernel, g_tree_converge_smem, m, plan, B, stream, m->dev, pr->P, plan,
-                             o_v, q, targets, task_mask, tol, (int)max_steps, q_out, err, steps, status, B);
+    const pk::ConvergeTreeLayout T = pk::converge_tree_layout(sel.plan);
+    return launch_tree_warps(pk::ik_tree_converge_kernel, g_tree_converge_smem, m, T.plan, B, stream, m->dev, pr->P,
+                             T.plan, T.o_v, q, targets, task_mask, tol, (int)max_steps, q_out, err, steps, status, B);
   }
-  const int block = 64;
-  const int64_t grid = (B + block - 1) / block;
-  pk::with_generic(sel.generic_class, [&](auto nj, auto nv) {
-    pk::ik_generic_converge_kernel<decltype(nj)::value, decltype(nv)::value><<<(unsigned)grid, block, 0, stream>>>(
-        m->dev, pr->P, q, targets, task_mask, tol, max_steps, q_out, err, steps, status, B);
+  return pk::with_generic(sel.generic_class, [&](auto nj, auto nv) {
+    return launch_rows(pk::ik_generic_converge_kernel<decltype(nj)::value, decltype(nv)::value>, B, 64, stream, m->dev,
+                       pr->P, q, targets, task_mask, tol, (int)max_steps, q_out, err, steps, status, B);
   });
-  return launched();
 }
 
 extern "C" int pk_converge_multistart_prepared(const PkModel* m, const PkProblem* pr, const float* q_seeds,
                                                int32_t num_seeds, const float* targets, uint32_t task_mask, float tol,
                                                int32_t max_steps, float* q_out, float* err, int32_t* seed,
                                                int32_t* steps, int32_t* status, int64_t B, void* stream_) {
-  if (check_common(m, q_seeds, B)) return 1;
-  if (!pr) return fail("null problem");
-  const std::string aerr = pk::check_converge_args(pr->P, task_mask, tol, max_steps);
-  if (!aerr.empty()) return fail(aerr);
-  const pk::Selection& sel = pr->sel;
-  const std::string serr = pk::check_multistart_seeds(sel, num_seeds);
-  if (!serr.empty()) return fail(serr);
-  const int S = num_seeds;
-  if (B > (int64_t)2147483647 * 32 / S) return fail("batch too large");
-  if (B > 0 && !q_out) return fail("null q_out");
-  if (B > 0 && pr->P.target_stride > 0 && !targets) return fail("null targets");
+  if (check_prepared(m, pr, q_seeds, targets, B, [&] {
+        const std::string aerr = pk::check_converge_args(pr->P, task_mask, tol, max_steps);
+        if (!aerr.empty()) return fail(aerr);
+        const std::string serr = pk::check_multistart_seeds(pr->sel, num_seeds);
+        if (!serr.empty()) return fail(serr);
+        if (B > (int64_t)2147483647 * 32 / num_seeds) return fail("batch too large");
+        return B > 0 && !q_out ? fail("null q_out") : 0;
+      }))
+    return 1;
   if (B == 0) return 0;
+  const pk::Selection& sel = pr->sel;
+  const int S = num_seeds;
   cudaStream_t stream = (cudaStream_t)stream_;
   if (sel.path == pk::kPathTree) {
     if (B > 2147483647) return fail("batch too large");
@@ -1217,28 +1160,19 @@ extern "C" int pk_converge_multistart_prepared(const PkModel* m, const PkProblem
                        m->dev, pr->P, T.plan, T.o_v, T.o_q, q_seeds, S, targets, task_mask, tol, (int)max_steps,
                        q_out, err, seed, steps, status, B);
   }
-  const int64_t rows = B * S;
   if (sel.path == pk::kPathChain) {
     const unsigned emask = pk::chain_task_mask(pr->P, task_mask, sel.nft);
-    const int block = 128;
-    const int64_t grid = (rows + block - 1) / block;
-    pk::with_nj(sel.nj, [&](auto nj) {
+    return pk::with_chain(sel, [&](auto nj, auto nft) {
       constexpr int NJ = decltype(nj)::value;
-      pk::with_nft(sel.nft, [&](auto nft) {
-        pk::ik_chain_multistart_kernel<NJ, decltype(nft)::value><<<(unsigned)grid, block, 0, stream>>>(
-            *reinterpret_cast<const pk::ChainParams<NJ>*>(pr->chain_params), q_seeds, S, targets, emask, tol,
-            max_steps, q_out, err, seed, steps, status, B);
-      });
+      return launch_rows(pk::ik_chain_multistart_kernel<NJ, decltype(nft)::value>, B * S, 128, stream, pr->chain<NJ>(),
+                         q_seeds, S, targets, emask, tol, (int)max_steps, q_out, err, seed, steps, status, B);
     });
-    return launched();
   }
-  const int block = 64;
-  const int64_t grid = (rows + block - 1) / block;
-  pk::with_generic(sel.generic_class, [&](auto nj, auto nv) {
-    pk::ik_generic_multistart_kernel<decltype(nj)::value, decltype(nv)::value><<<(unsigned)grid, block, 0, stream>>>(
-        m->dev, pr->P, q_seeds, S, targets, task_mask, tol, max_steps, q_out, err, seed, steps, status, B);
+  return pk::with_generic(sel.generic_class, [&](auto nj, auto nv) {
+    return launch_rows(pk::ik_generic_multistart_kernel<decltype(nj)::value, decltype(nv)::value>, B * S, 64, stream,
+                       m->dev, pr->P, q_seeds, S, targets, task_mask, tol, (int)max_steps, q_out, err, seed, steps,
+                       status, B);
   });
-  return launched();
 }
 
 extern "C" int pk_solve_ik_batched(const PkModel* m, const PkProblemDesc* prob, const float* q,
@@ -1506,9 +1440,5 @@ extern "C" int pk_integrate_batched(const PkModel* m, const float* q, const floa
   if (check_common(m, q, B)) return 1;
   if (B == 0) return 0;
   if (!v || !q_out) return fail("null v or q_out");
-  const int block = 128;
-  const int64_t grid = (B + block - 1) / block;
-  pk::integrate_kernel<<<(unsigned)grid, block, 0, (cudaStream_t)stream>>>(m->nq, m->nv, m->free_flyer, q, v, dt,
-                                                                             q_out, B);
-  return launched();
+  return launch_rows(pk::integrate_kernel, B, 128, (cudaStream_t)stream, m->nq, m->nv, m->free_flyer, q, v, dt, q_out, B);
 }

@@ -341,6 +341,26 @@ PK_HD void converge_chain(const ChainParams<NJ>& P, float (&q)[NJ], const float*
   status_out = st_all;
 }
 
+// Instance i of ik_chain_converge_kernel: converge_chain from q row i, where it stopped into q_out
+// row i, then err, steps and status (each unless null).  q_out may alias q (the row is read before
+// it is written).
+template <int NJ, int NFT>
+PK_HD void converge_chain_instance(const ChainParams<NJ>& P, const float* q, const float* __restrict__ targets,
+                                   unsigned emask, float tol, int max_steps, float* q_out, float* __restrict__ err,
+                                   int32_t* __restrict__ steps, int32_t* __restrict__ status, int64_t i) {
+  float qi[NJ];
+#pragma unroll
+  for (int k = 0; k < NJ; ++k) qi[k] = q[i * NJ + k];
+  float e;
+  int n, st;
+  converge_chain<NJ, NFT>(P, qi, targets + i * (int64_t)P.target_stride, emask, tol, max_steps, e, n, st);
+#pragma unroll
+  for (int k = 0; k < NJ; ++k) q_out[i * NJ + k] = qi[k];
+  if (err) err[i] = e;
+  if (steps) steps[i] = n;
+  if (status) status[i] = st;
+}
+
 // Records of step s of a trajectory (thread-per-instance chain kernel); `frozen`: v row of zeros.
 template <int NJ>
 PK_HD void chain_record(const Trajectory& T, int s, int64_t B, int64_t i, const float (&qi)[NJ],

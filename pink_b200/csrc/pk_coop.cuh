@@ -736,4 +736,58 @@ PK_HD int rollout_coop(const Group<L>& G, const CoopParams<CoopStep<NJ, NFT, L>:
   return st_all;
 }
 
+// Instance `inst` of ik_coop_kernel: its q row into the lanes (padding joints at zero), rollout_coop,
+// then each lane stores the joints it owns of v and of q_out (unless null), lane 0 of the group the
+// status (unless null).
+template <int NJ, int NFT, int L, class JC>
+PK_HD void coop_instance(const Group<L>& G, const CoopParams<CoopStep<NJ, NFT, L>::NJP>& P, JC jc,
+                         const float* __restrict__ q, const float* __restrict__ targets, float* __restrict__ v,
+                         int32_t* __restrict__ status, int64_t B, int n_steps, float* __restrict__ q_out,
+                         const Trajectory& T, int64_t inst) {
+  using Step = CoopStep<NJ, NFT, L>;
+  constexpr int NC = Step::NC;
+  GVar<typename Step::Lane, L> S;
+  const float* qrow = q + inst * NJ;
+  PK_GLANES(G, h) {
+    if constexpr (L == 1 && NJ % 2 == 0) {
+#pragma unroll
+      for (int k = 0; k < NJ / 2; ++k) {
+        const float2 t = load_ro(reinterpret_cast<const float2*>(qrow) + k);
+        S[h].q[2 * k] = t.x;
+        S[h].q[2 * k + 1] = t.y;
+      }
+    } else {
+#pragma unroll
+      for (int k = 0; k < NC; ++k) {
+        const int j = h * NC + k;
+        S[h].q[k] = (j < NJ) ? load_ro(qrow + (j < NJ ? j : 0)) : 0.f;
+      }
+    }
+  }
+  const int st_all = rollout_coop<NJ, NFT, L>(G, P, jc, targets + inst * (int64_t)P.target_stride, S, n_steps,
+                                              q_out != nullptr, T, B, inst);
+  float* vrow = v + inst * NJ;
+  PK_GLANES(G, h) {
+    if constexpr (L == 1 && NJ % 2 == 0) {
+#pragma unroll
+      for (int k = 0; k < NJ / 2; ++k) reinterpret_cast<float2*>(vrow)[k] = make_float2(S[h].x[2 * k], S[h].x[2 * k + 1]);
+    } else {
+#pragma unroll
+      for (int k = 0; k < NC; ++k) {
+        const int j = h * NC + k;
+        if (j < NJ) vrow[j] = S[h].x[k];
+      }
+    }
+    if (q_out) {
+      float* orow = q_out + inst * NJ;
+#pragma unroll
+      for (int k = 0; k < NC; ++k) {
+        const int j = h * NC + k;
+        if (j < NJ) orow[j] = S[h].q[k];
+      }
+    }
+    if (status && h == 0) status[inst] = st_all;
+  }
+}
+
 }  // namespace pk

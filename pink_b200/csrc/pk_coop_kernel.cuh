@@ -25,7 +25,6 @@ __global__ void __launch_bounds__(kCoopThreads, CoopOccupancy<L>::min_blocks)
                    const float* __restrict__ targets, float* __restrict__ v, int32_t* __restrict__ status,
                    int64_t B, int n_steps, float* __restrict__ q_out, const __grid_constant__ Trajectory T) {
   using Step = CoopStep<NJ, NFT, L>;
-  constexpr int NC = Step::NC;
   // lane-varying joint index (L > 1): the per-joint constants come from shared memory
   __shared__ CoopJoint sj[L > 1 ? Step::NJP : 1];
   if constexpr (L > 1) {
@@ -42,44 +41,7 @@ __global__ void __launch_bounds__(kCoopThreads, CoopOccupancy<L>::min_blocks)
     if constexpr (L > 1) return sj[j];
     else return P.joint[j];
   };
-  GVar<typename Step::Lane, L> S;
-  const float* qrow = q + inst * NJ;
-  if constexpr (L == 1 && NJ % 2 == 0) {
-#pragma unroll
-    for (int k = 0; k < NJ / 2; ++k) {
-      const float2 t = __ldg(reinterpret_cast<const float2*>(qrow) + k);
-      S.v.q[2 * k] = t.x;
-      S.v.q[2 * k + 1] = t.y;
-    }
-  } else {
-#pragma unroll
-    for (int k = 0; k < NC; ++k) {
-      const int j = G.h * NC + k;
-      S.v.q[k] = (j < NJ) ? __ldg(qrow + (j < NJ ? j : 0)) : 0.f;
-    }
-  }
-  const int st_all = rollout_coop<NJ, NFT, L>(G, P, jc, targets + inst * (int64_t)P.target_stride, S, n_steps,
-                                              q_out != nullptr, T, B, inst);
-  float* vrow = v + inst * NJ;
-  if constexpr (L == 1 && NJ % 2 == 0) {
-#pragma unroll
-    for (int k = 0; k < NJ / 2; ++k) reinterpret_cast<float2*>(vrow)[k] = make_float2(S.v.x[2 * k], S.v.x[2 * k + 1]);
-  } else {
-#pragma unroll
-    for (int k = 0; k < NC; ++k) {
-      const int j = G.h * NC + k;
-      if (j < NJ) vrow[j] = S.v.x[k];
-    }
-  }
-  if (q_out) {
-    float* orow = q_out + inst * NJ;
-#pragma unroll
-    for (int k = 0; k < NC; ++k) {
-      const int j = G.h * NC + k;
-      if (j < NJ) orow[j] = S.v.q[k];
-    }
-  }
-  if (status && G.h == 0) status[inst] = st_all;
+  coop_instance<NJ, NFT, L>(G, P, jc, q, targets, v, status, B, n_steps, q_out, T, inst);
 }
 
 }  // namespace pk

@@ -790,4 +790,39 @@ PK_HD int rollout_generic(Generic<NJMAX, NVMAX>& G, const DevModel& M, const Dev
   return st_all;
 }
 
+// Instance i of ik_generic_rollout_kernel: q row i into q_out row i, rollout_generic there in place
+// with v row i, then the status (unless null).
+template <int NJMAX, int NVMAX>
+PK_HD void rollout_generic_instance(Generic<NJMAX, NVMAX>& G, const DevModel& M, const DevProblem& P, const float* q,
+                                    const float* __restrict__ targets, int n_steps, float* q_out,
+                                    float* __restrict__ v, int32_t* __restrict__ status, const Trajectory& T,
+                                    int64_t B, int64_t i) {
+  const int nq = M.nq;
+  float* qrow = q_out + i * nq;
+  for (int k = 0; k < nq; ++k) qrow[k] = q[i * nq + k];
+  const int st_all = rollout_generic(G, M, P, qrow, v + i * M.nv, targets, n_steps, T, B, i);
+  if (status) status[i] = st_all;
+}
+
+// Instance i of ik_generic_converge_kernel: q row i into q_out row i (q_out may alias q),
+// converge_generic there in place with v in local memory, then err, steps and status (each unless
+// null).
+template <int NJMAX, int NVMAX>
+PK_HD void converge_generic_instance(Generic<NJMAX, NVMAX>& G, const DevModel& M, const DevProblem& P, const float* q,
+                                     const float* __restrict__ targets, unsigned mask, float tol, int max_steps,
+                                     float* q_out, float* __restrict__ err, int32_t* __restrict__ steps,
+                                     int32_t* __restrict__ status, int64_t i) {
+  const int nq = M.nq;
+  float* qrow = q_out + i * nq;
+  for (int k = 0; k < nq; ++k) qrow[k] = q[i * nq + k];
+  float v[NVMAX];
+  float e;
+  int n, st;
+  converge_generic(G, M, P, qrow, targets ? targets + i * (int64_t)P.target_stride : nullptr, v, mask, tol, max_steps,
+                   e, n, st);
+  if (err) err[i] = e;
+  if (steps) steps[i] = n;
+  if (status) status[i] = st;
+}
+
 }  // namespace pk

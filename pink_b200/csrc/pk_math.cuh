@@ -24,8 +24,10 @@
 #endif
 
 #if !defined(__CUDACC__)
-// host-only build (tests/hostsim): glibc has no rsqrtf
+// host-only build (tests/hostsim): glibc has no rsqrtf, and no CUDA vector types
 static inline float rsqrtf(float x) { return 1.0f / sqrtf(x); }
+struct float2 { float x, y; };
+static inline float2 make_float2(float x, float y) { return float2{x, y}; }
 #endif
 
 namespace pk {
@@ -123,6 +125,16 @@ PK_HD SE3f load_se3(const float* t) {  // 12 floats, row-major [R | p]
   T.R.m[6] = t[8]; T.R.m[7] = t[9]; T.R.m[8] = t[10]; T.p.z = t[11];
   return T;
 }
+// *p for an input the kernel never writes: through the read-only data cache on the device
+template <class T>
+PK_HD T load_ro(const T* p) {
+#if defined(__CUDA_ARCH__)
+  return __ldg(p);
+#else
+  return *p;
+#endif
+}
+
 // 12 floats; `vec4`: the address is 16-byte aligned (three 128-bit read-only loads instead
 // of twelve scalar ones when it is in global memory)
 PK_HD SE3f load_se3_vec4(const float* t, bool vec4) {

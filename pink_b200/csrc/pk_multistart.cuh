@@ -1,7 +1,7 @@
 // Multi-start solve to a tolerance (pk_converge_multistart_prepared): each target is solved
 // from S seeds at once, and the group of S seeds stops at the first round where one of them
-// has converged.  Device code only; the host build (tests/hostsim/multistart.cpp) runs the
-// same step bodies in two passes per round.
+// has converged.  Device code only; the host build (hs_converge_multistart in hostsim.cpp) runs
+// the same step bodies in two passes per round.
 //
 // The S seeds of a target advance in lockstep rounds s = 0, 1, ...: every seed that has not
 // failed computes err(q_s) (the error of converge); the group stops when some seed has

@@ -73,23 +73,30 @@ inline unsigned chain_task_mask(const DevProblem& P, unsigned mask, int nft) {
   return out;
 }
 
+// Solve to a tolerance on joint trees (pk_converge_prepared): a warp's workspace is the plan's
+// words, then the step's v (4-word aligned).
+struct ConvergeTreeLayout {
+  TreePlan plan;  // plan.words: the whole per-warp workspace
+  int o_v;
+};
+inline ConvergeTreeLayout converge_tree_layout(const TreePlan& plan) {
+  ConvergeTreeLayout T{plan, plan.words};
+  T.plan.words += (plan.nv + 3) & ~3;
+  return T;
+}
+
 // Multi-start on joint trees (pk_converge_multistart_prepared): one target per CTA, one seed per
-// warp.  A warp's workspace is the plan's words, then the step's v, then the seed's q (each
-// 4-word aligned); after the S workspaces come the group's slots, two rounds of S errors and S
-// failed flags.  The CTA's dynamic shared memory is capped at kCtaSmemBytes, the opt-in limit of
-// sm_90.
+// warp.  A warp's workspace is converge's, then the seed's q (4-word aligned); after the S
+// workspaces come the group's slots, two rounds of S errors and S failed flags.  The CTA's
+// dynamic shared memory is capped at kCtaSmemBytes, the opt-in limit of sm_90.
 constexpr int kTreeMaxSeeds = 8;
 constexpr size_t kCtaSmemBytes = 227 * 1024;
-struct MultistartTreeLayout {
-  TreePlan plan;  // plan.words: the whole per-warp workspace
-  int o_v, o_q;
+struct MultistartTreeLayout : ConvergeTreeLayout {
+  int o_q;
   size_t smem_bytes(int S) const { return ((size_t)plan.words * S + 4 * (size_t)S) * 4; }
 };
 inline MultistartTreeLayout multistart_tree_layout(const TreePlan& plan) {
-  MultistartTreeLayout T;
-  T.plan = plan;
-  T.o_v = T.plan.words;
-  T.plan.words += (plan.nv + 3) & ~3;
+  MultistartTreeLayout T{converge_tree_layout(plan), 0};
   T.o_q = T.plan.words;
   T.plan.words += (plan.nq + 3) & ~3;
   return T;
@@ -132,6 +139,12 @@ decltype(auto) with_nft(int nft, F&& f) {
     case 1: return f(std::integral_constant<int, 1>{});
     default: return f(std::integral_constant<int, 2>{});
   }
+}
+
+// f(<NJ>, <NFT>) for a chain selection
+template <class F>
+decltype(auto) with_chain(const Selection& sel, F&& f) {
+  return with_nj(sel.nj, [&](auto nj) { return with_nft(sel.nft, [&](auto nft) { return f(nj, nft); }); });
 }
 
 template <int NJ, int NFT, class F>

@@ -1230,6 +1230,51 @@ struct TreeStep {
       PK_LANES(l) record_rows(T, s, B, i, L.nq, L.nv, qg, vg, st_all, true, l, 32);
     return st_all;
   }
+
+  // Instance i of the one-instance-per-warp kernels, W its warp's workspace.  ik_tree_kernel: run on
+  // q row i into v row i and status[i] (unless null).
+  static PK_HD void solve_instance(const DevModel& M, const DevProblem& P, const TreePlan& L, const float* __restrict__ q,
+                                   const float* __restrict__ targets, float* W, float* __restrict__ v,
+                                   int32_t* __restrict__ status, int64_t i) {
+    run(M, P, L, q + i * L.nq, targets ? targets + i * (int64_t)L.stride : nullptr, W, v + i * L.nv,
+        status ? status + i : nullptr);
+  }
+
+  // ik_tree_rollout_kernel: q row i into q_out row i, rollout there in place with v row i, then the
+  // status (unless null).
+  static PK_HD void rollout_instance(const DevModel& M, const DevProblem& P, const TreePlan& L,
+                                     const float* __restrict__ q, const float* __restrict__ targets, int n_steps,
+                                     float* __restrict__ q_out, float* W, float* __restrict__ v,
+                                     int32_t* __restrict__ status, const Trajectory& T, int64_t B, int64_t i) {
+    float* qrow = q_out + i * L.nq;
+    PK_LANES(l) for (int k = l; k < L.nq; k += 32) qrow[k] = q[i * L.nq + k];
+    PK_WSYNC();
+    const int st_all = rollout(M, P, L, qrow, targets, W, v + i * L.nv, n_steps, T, B, i);
+    PK_LANES(l) if (status && l == 0) status[i] = st_all;
+  }
+
+  // ik_tree_converge_kernel: q row i into q_out row i (q_out may alias q), converge there in place
+  // with the step's v at word o_v of W (converge_tree_layout), then err, steps and status (each
+  // unless null).
+  static PK_HD void converge_instance(const DevModel& M, const DevProblem& P, const TreePlan& L, int o_v,
+                                      const float* q, const float* __restrict__ targets, unsigned mask, float tol,
+                                      int max_steps, float* q_out, float* W, float* __restrict__ err,
+                                      int32_t* __restrict__ steps, int32_t* __restrict__ status, int64_t i) {
+    float* qrow = q_out + i * L.nq;
+    PK_LANES(l) for (int k = l; k < L.nq; k += 32) qrow[k] = q[i * L.nq + k];
+    PK_WSYNC();
+    float e;
+    int n, st;
+    converge(M, P, L, qrow, targets ? targets + i * (int64_t)L.stride : nullptr, W, W + o_v, mask, tol, max_steps, e,
+             n, st);
+    PK_LANES(l) {
+      if (l == 0) {
+        if (err) err[i] = e;
+        if (steps) steps[i] = n;
+        if (status) status[i] = st;
+      }
+    }
+  }
 };
 
 }  // namespace pk

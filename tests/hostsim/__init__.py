@@ -1,6 +1,9 @@
 """ctypes wrapper of ``libpk_hostsim.so``: the kernel bodies of
-``pink_b200/csrc`` and their rollout, converge and multi-start loops compiled for the host CPU
-(see hostsim.cpp).
+``pink_b200/csrc`` compiled for the host CPU (see hostsim.cpp).  Each entry makes the problem,
+runs the library's kernel selection and loops over the instances with the body the selection
+names: the per-instance bodies the kernels call (indexing, loads, rollout / converge loop,
+stores), the step bodies for the chain solve and the general path, and the two-pass rounds of
+multi-start.
 
 TEST HARNESS ONLY.  The product package never imports this module; it exists
 so that the CPU test-suite can run the kernels' exact fp32 arithmetic against

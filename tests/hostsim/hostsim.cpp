@@ -1,8 +1,9 @@
-// CPU build of the kernel bodies (pk_chain.cuh / pk_generic.cuh) for the test suite
-// ONLY: lets `pytest -m "not gpu"` exercise the exact fp32 arithmetic and
-// control flow of the CUDA kernels against the fp64 oracle on machines without
-// a GPU.  It is never loaded by the product package (pink_b200/_cabi.py loads
-// libpink_b200.so and nothing else) and is not a fallback.
+// CPU build of the kernel bodies (pink_b200/csrc) for the test suite ONLY: lets
+// `pytest -m "not gpu"` exercise the exact fp32 arithmetic and control flow of the
+// CUDA kernels against the fp64 oracle on machines without a GPU.  Each entry makes the
+// problem, selects (pk_select.hpp) and loops over the instances with the per-instance body
+// the selected kernel calls.  It is never loaded by the product package (pink_b200/_cabi.py
+// loads libpink_b200.so and nothing else) and is not a fallback.
 #include <cmath>
 #include <cstdint>
 #include <cstring>
@@ -53,66 +54,26 @@ float* tree_workspace(std::vector<float>& W, int words) {
   return ((uintptr_t)p & 7) != 0 ? p + 1 : p;
 }
 
-// The chain kernel a chain selection names: chain(C) with the thread-per-instance kernel's
-// parameter block, or coop(lanes, C, jc) with the sub-warp kernel's (lanes emulated by loops).
-template <int NJ, int NFT, class Chain, class Coop>
+// The chain kernel a chain selection names, at its <NJ, NFT>: chain(nj, nft, C) with the
+// thread-per-instance kernel's parameter block, or coop(nj, nft, G, C, jc) with the sub-warp
+// kernel's (a group of lanes emulated by loops).
+template <class Chain, class Coop>
 void with_chain_kernel(const pk::HostModel& hm, const pk::DevProblem& P, const pk::Selection& sel, Chain chain,
                        Coop coop) {
-  if (!sel.lanes) {
-    pk::ChainParams<NJ> C;
-    pk::make_chain_params<NJ>(hm, P, &C, P.ext);
-    return chain(C);
-  }
-  pk::with_lanes<NJ, NFT>(sel.lanes, [&](auto lanes) {
-    typename pk::CoopStep<NJ, NFT, decltype(lanes)::value>::Params C;
-    pk::make_coop_params<NJ, decltype(lanes)::value>(hm, P, &C, P.ext);
-    coop(lanes, C, [&](int j) -> const pk::CoopJoint& { return C.joint[j]; });
+  pk::with_chain(sel, [&](auto nj, auto nft) {
+    constexpr int NJ = decltype(nj)::value, NFT = decltype(nft)::value;
+    if (!sel.lanes) {
+      pk::ChainParams<NJ> C;
+      pk::make_chain_params<NJ>(hm, P, &C, P.ext);
+      return chain(nj, nft, C);
+    }
+    pk::with_lanes<NJ, NFT>(sel.lanes, [&](auto lanes) {
+      constexpr int L = decltype(lanes)::value;
+      typename pk::CoopStep<NJ, NFT, L>::Params C;
+      pk::make_coop_params<NJ, L>(hm, P, &C, P.ext);
+      coop(nj, nft, pk::Group<L>{}, C, [&](int j) -> const pk::CoopJoint& { return C.joint[j]; });
+    });
   });
-}
-
-// Instance i's q row into the lanes of the sub-warp kernel (padding joints at zero), and back:
-// the lanes' q into q_out row i (unless null) and their velocity into v row i.
-template <int NJ, int NC, int L, class Lane>
-void coop_load(pk::GVar<Lane, L>& S, const float* q, int64_t i) {
-  for (int h = 0; h < L; ++h)
-    for (int k = 0; k < NC; ++k) S[h].q[k] = h * NC + k < NJ ? q[i * NJ + h * NC + k] : 0.f;
-}
-template <int NJ, int NC, int L, class Lane>
-void coop_store(const pk::GVar<Lane, L>& S, float* q_out, float* v, int64_t i) {
-  for (int h = 0; h < L; ++h)
-    for (int k = 0; k < NC && h * NC + k < NJ; ++k) {
-      if (q_out) q_out[i * NJ + h * NC + k] = S[h].q[k];
-      v[i * NJ + h * NC + k] = S[h].x[k];
-    }
-}
-
-// The bodies of the kernels a chain selection names.
-template <int NJ, int NFT>
-void run_chain(const pk::HostModel& hm, const pk::DevProblem& P, const pk::Selection& sel, const float* q,
-               const float* targets, float* v, int32_t* status, int64_t B) {
-  auto chain = [&](const pk::ChainParams<NJ>& C) {
-    for (int64_t i = 0; i < B; ++i) {
-      float qi[NJ], vi[NJ];
-      for (int k = 0; k < NJ; ++k) qi[k] = q[i * NJ + k];
-      int st = 0;
-      pk::ik_step_chain<NJ, NFT>(C, qi, targets + i * (int64_t)P.target_stride, vi, st);
-      for (int k = 0; k < NJ; ++k) v[i * NJ + k] = vi[k];
-      if (status) status[i] = st;
-    }
-  };
-  auto coop = [&](auto lanes, const auto& C, auto jc) {
-    constexpr int L = decltype(lanes)::value;
-    using Step = pk::CoopStep<NJ, NFT, L>;
-    for (int64_t i = 0; i < B; ++i) {
-      pk::GVar<typename Step::Lane, L> S;
-      coop_load<NJ, Step::NC>(S, q, i);
-      int st = 0;
-      pk::ik_step_coop<NJ, NFT, L>(pk::Group<L>{}, C, jc, targets + i * (int64_t)P.target_stride, S, st);
-      coop_store<NJ, Step::NC>(S, nullptr, v, i);
-      if (status) status[i] = st;
-    }
-  };
-  with_chain_kernel<NJ, NFT>(hm, P, sel, chain, coop);
 }
 
 // ik_generic_kernel's body at the instantiation the CUDA library launches for this model
@@ -176,19 +137,29 @@ int hs_solve_ik(void* model, const PkProblemDesc* prob, const float* q, const fl
   const std::string serr = select(hm, P, hx, path, true, sel_out, &sel);
   if (!serr.empty()) return fail(serr);
   if (sel.path == pk::kPathChain) {
-    pk::with_nj(sel.nj, [&](auto nj) {
-      pk::with_nft(sel.nft, [&](auto nft) {
-        run_chain<decltype(nj)::value, decltype(nft)::value>(hm, P, sel, q, targets, v, status, B);
-      });
-    });
+    with_chain_kernel(
+        hm, P, sel,
+        [&](auto nj, auto nft, const auto& C) {
+          constexpr int NJ = decltype(nj)::value;
+          for (int64_t i = 0; i < B; ++i) {
+            float qi[NJ], vi[NJ];
+            for (int k = 0; k < NJ; ++k) qi[k] = q[i * NJ + k];
+            int st = 0;
+            pk::ik_step_chain<NJ, decltype(nft)::value>(C, qi, targets + i * (int64_t)P.target_stride, vi, st);
+            for (int k = 0; k < NJ; ++k) v[i * NJ + k] = vi[k];
+            if (status) status[i] = st;
+          }
+        },
+        [&](auto nj, auto nft, auto G, const auto& C, auto jc) {
+          for (int64_t i = 0; i < B; ++i)
+            pk::coop_instance<decltype(nj)::value, decltype(nft)::value>(G, C, jc, q, targets, v, status, B, 1, nullptr,
+                                                                         pk::Trajectory{}, i);
+        });
   } else if (sel.path == pk::kPathTree) {
-    const pk::TreePlan& L = sel.plan;
     const pk::DevModel M = hm.host_view();
     std::vector<float> W;
-    float* Wp = tree_workspace(W, L.words);
-    for (int64_t i = 0; i < B; ++i)
-      pk::TreeStep::run(M, P, L, q + i * L.nq, targets ? targets + i * (int64_t)L.stride : nullptr, Wp,
-                        v + i * L.nv, status ? status + i : nullptr);
+    float* Wp = tree_workspace(W, sel.plan.words);
+    for (int64_t i = 0; i < B; ++i) pk::TreeStep::solve_instance(M, P, sel.plan, q, targets, Wp, v, status, i);
   } else {
     pk::GenericArgs A{};
     A.q = q; A.targets = targets; A.v = v; A.status = status; A.task_index = -1;
@@ -214,57 +185,34 @@ int hs_rollout(void* model, const PkProblemDesc* prob, const float* q, const flo
   if (!serr.empty()) return fail(serr);
   const pk::Trajectory T{target_step, q_traj, v_traj, status_traj};
   const pk::DevModel M = hm.host_view();
-  const int nq = hm.nq, nv = hm.nv;
-  auto start = [&](int64_t i) {
-    float* qrow = q_out + i * nq;
-    std::memcpy(qrow, q + i * nq, sizeof(float) * nq);
-    return qrow;
-  };
   if (sel.path == pk::kPathChain) {
-    pk::with_nj(sel.nj, [&](auto nj) {
-      constexpr int NJ = decltype(nj)::value;
-      pk::with_nft(sel.nft, [&](auto nft) {
-        constexpr int NFT = decltype(nft)::value;
-        auto chain = [&](const pk::ChainParams<NJ>& C) {
+    with_chain_kernel(
+        hm, P, sel,
+        [&](auto nj, auto nft, const auto& C) {
+          constexpr int NJ = decltype(nj)::value;
           for (int64_t i = 0; i < B; ++i) {
             float qi[NJ], vi[NJ];
             for (int k = 0; k < NJ; ++k) qi[k] = q[i * NJ + k];
-            const int st_all = pk::rollout_chain<NJ, NFT, true>(C, qi, targets + i * (int64_t)P.target_stride, vi,
-                                                                n_steps, true, 0, T, B, i);
+            const int st_all = pk::rollout_chain<NJ, decltype(nft)::value, true>(
+                C, qi, targets + i * (int64_t)P.target_stride, vi, n_steps, true, 0, T, B, i);
             for (int k = 0; k < NJ; ++k) { q_out[i * NJ + k] = qi[k]; v[i * NJ + k] = vi[k]; }
             if (status) status[i] = st_all;
           }
-        };
-        auto coop = [&](auto lanes, const auto& C, auto jc) {
-          constexpr int L = decltype(lanes)::value;
-          using Step = pk::CoopStep<NJ, NFT, L>;
-          for (int64_t i = 0; i < B; ++i) {
-            pk::GVar<typename Step::Lane, L> S;
-            coop_load<NJ, Step::NC>(S, q, i);
-            const int st_all = pk::rollout_coop<NJ, NFT, L>(pk::Group<L>{}, C, jc,
-                                                            targets + i * (int64_t)P.target_stride, S, n_steps, true,
-                                                            T, B, i);
-            coop_store<NJ, Step::NC>(S, q_out, v, i);
-            if (status) status[i] = st_all;
-          }
-        };
-        with_chain_kernel<NJ, NFT>(hm, P, sel, chain, coop);
-      });
-    });
+        },
+        [&](auto nj, auto nft, auto G, const auto& C, auto jc) {
+          for (int64_t i = 0; i < B; ++i)
+            pk::coop_instance<decltype(nj)::value, decltype(nft)::value>(G, C, jc, q, targets, v, status, B, n_steps,
+                                                                         q_out, T, i);
+        });
   } else if (sel.path == pk::kPathTree) {
     std::vector<float> W;
     float* Wp = tree_workspace(W, sel.plan.words);
-    for (int64_t i = 0; i < B; ++i) {
-      const int st_all = pk::TreeStep::rollout(M, P, sel.plan, start(i), targets, Wp, v + i * nv, n_steps, T, B, i);
-      if (status) status[i] = st_all;
-    }
+    for (int64_t i = 0; i < B; ++i)
+      pk::TreeStep::rollout_instance(M, P, sel.plan, q, targets, n_steps, q_out, Wp, v, status, T, B, i);
   } else {
-    pk::with_generic(sel.generic_class, [&](auto nj, auto nvm) {
-      static thread_local pk::Generic<decltype(nj)::value, decltype(nvm)::value> G;
-      for (int64_t i = 0; i < B; ++i) {
-        const int st_all = pk::rollout_generic(G, M, P, start(i), v + i * nv, targets, n_steps, T, B, i);
-        if (status) status[i] = st_all;
-      }
+    pk::with_generic(sel.generic_class, [&](auto nj, auto nv) {
+      static thread_local pk::Generic<decltype(nj)::value, decltype(nv)::value> G;
+      for (int64_t i = 0; i < B; ++i) pk::rollout_generic_instance(G, M, P, q, targets, n_steps, q_out, v, status, T, B, i);
     });
   }
   return 0;
@@ -288,51 +236,28 @@ int hs_converge(void* model, const PkProblemDesc* prob, const float* q, const fl
   const std::string serr = select(hm, P, hx, path, true, sel_out, &sel);
   if (!serr.empty()) return fail(serr);
   const pk::DevModel M = hm.host_view();
-  const int nq = hm.nq;
-  auto trow = [&](int64_t i) { return targets ? targets + i * (int64_t)P.target_stride : nullptr; };
-  auto start = [&](int64_t i) {
-    float* qrow = q_out + i * nq;
-    if (qrow != q + i * nq) std::memcpy(qrow, q + i * nq, sizeof(float) * nq);
-    return qrow;
-  };
-  auto store = [&](int64_t i, float ei, int n, int st) {
-    if (err) err[i] = ei;
-    if (steps) steps[i] = n;
-    if (status) status[i] = st;
-  };
-  float ei;
-  int n, st;
   if (sel.path == pk::kPathChain) {
-    pk::with_nj(sel.nj, [&](auto nj) {
+    const unsigned emask = pk::chain_task_mask(P, mask, sel.nft);
+    pk::with_chain(sel, [&](auto nj, auto nft) {
       constexpr int NJ = decltype(nj)::value;
       pk::ChainParams<NJ> C;
       pk::make_chain_params<NJ>(hm, P, &C, P.ext);
-      const unsigned emask = pk::chain_task_mask(P, mask, sel.nft);
-      pk::with_nft(sel.nft, [&](auto nft) {
-        for (int64_t i = 0; i < B; ++i) {
-          float qi[NJ];
-          for (int k = 0; k < NJ; ++k) qi[k] = q[i * NJ + k];
-          pk::converge_chain<NJ, decltype(nft)::value>(C, qi, trow(i), emask, tol, max_steps, ei, n, st);
-          for (int k = 0; k < NJ; ++k) q_out[i * NJ + k] = qi[k];
-          store(i, ei, n, st);
-        }
-      });
+      for (int64_t i = 0; i < B; ++i)
+        pk::converge_chain_instance<NJ, decltype(nft)::value>(C, q, targets, emask, tol, max_steps, q_out, err, steps,
+                                                              status, i);
     });
   } else if (sel.path == pk::kPathTree) {
-    std::vector<float> W, v(hm.nv);
-    float* Wp = tree_workspace(W, sel.plan.words);
-    for (int64_t i = 0; i < B; ++i) {
-      pk::TreeStep::converge(M, P, sel.plan, start(i), trow(i), Wp, v.data(), mask, tol, max_steps, ei, n, st);
-      store(i, ei, n, st);
-    }
+    const pk::ConvergeTreeLayout T = pk::converge_tree_layout(sel.plan);
+    std::vector<float> W;
+    float* Wp = tree_workspace(W, T.plan.words);
+    for (int64_t i = 0; i < B; ++i)
+      pk::TreeStep::converge_instance(M, P, T.plan, T.o_v, q, targets, mask, tol, max_steps, q_out, Wp, err, steps,
+                                      status, i);
   } else {
     pk::with_generic(sel.generic_class, [&](auto nj, auto nv) {
       static thread_local pk::Generic<decltype(nj)::value, decltype(nv)::value> G;
-      float v[decltype(nv)::value];
-      for (int64_t i = 0; i < B; ++i) {
-        pk::converge_generic(G, M, P, start(i), trow(i), v, mask, tol, max_steps, ei, n, st);
-        store(i, ei, n, st);
-      }
+      for (int64_t i = 0; i < B; ++i)
+        pk::converge_generic_instance(G, M, P, q, targets, mask, tol, max_steps, q_out, err, steps, status, i);
     });
   }
   return 0;
@@ -375,30 +300,27 @@ int hs_converge_multistart(void* model, const PkProblemDesc* prob, const float* 
     std::fill(st_all.begin(), st_all.end(), 0);
     int w = 0, n = 0;
     if (sel.path == pk::kPathChain) {
-      pk::with_nj(sel.nj, [&](auto nj) {
-        constexpr int NJ = decltype(nj)::value;
+      const unsigned emask = pk::chain_task_mask(P, mask, sel.nft);
+      pk::with_chain(sel, [&](auto nj, auto nft) {
+        constexpr int NJ = decltype(nj)::value, NFT = decltype(nft)::value;
         pk::ChainParams<NJ> C;
         pk::make_chain_params<NJ>(hm, P, &C, P.ext);
-        const unsigned emask = pk::chain_task_mask(P, mask, sel.nft);
-        pk::with_nft(sel.nft, [&](auto nft) {
-          constexpr int NFT = decltype(nft)::value;
-          auto qj = [&](int j) -> float(&)[NJ] { return *reinterpret_cast<float(*)[NJ]>(qs.data() + j * NJ); };
-          auto error = [&](int j) {
-            pk::ChainStep<NJ, NFT> Cs;
-            bool skip;
-            float ej;
-            Cs.template assemble<true>(C, qj(j), trow, skip, emask, &ej);
-            return ej;
-          };
-          auto advance = [&](int j) {
-            pk::ChainStep<NJ, NFT> Cs;
-            bool skip;
-            float ej;
-            const int st = Cs.template assemble<true>(C, qj(j), trow, skip, emask, &ej);
-            return pk::converge_chain_advance(C, Cs, st, skip, qj(j), st_all[j], 0);
-          };
-          w = run_group(S, tol, max_steps, error, advance, es, n);
-        });
+        auto qj = [&](int j) -> float(&)[NJ] { return *reinterpret_cast<float(*)[NJ]>(qs.data() + j * NJ); };
+        auto error = [&](int j) {
+          pk::ChainStep<NJ, NFT> Cs;
+          bool skip;
+          float ej;
+          Cs.template assemble<true>(C, qj(j), trow, skip, emask, &ej);
+          return ej;
+        };
+        auto advance = [&](int j) {
+          pk::ChainStep<NJ, NFT> Cs;
+          bool skip;
+          float ej;
+          const int st = Cs.template assemble<true>(C, qj(j), trow, skip, emask, &ej);
+          return pk::converge_chain_advance(C, Cs, st, skip, qj(j), st_all[j], 0);
+        };
+        w = run_group(S, tol, max_steps, error, advance, es, n);
       });
     } else if (sel.path == pk::kPathTree) {
       const pk::TreePlan& L = sel.plan;
