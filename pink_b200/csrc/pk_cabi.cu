@@ -325,11 +325,14 @@ __device__ __forceinline__ void peer_count_kernel(const PeerOut& peers) {
 //   - the library cannot see what ran before it on the stream (our own previous call
 //     writing this call's q, or a foreign kernel that triggers early and then writes q or
 //     the targets), so after the wait the q row and the targets row are read again from L2
-//     (ld.global.cg) and compared bitwise with the values the steps used.  On a difference
-//     every step of the instance is recomputed from the re-read values.
-// The steps read the targets row from a copy in local memory, never through the read-only
-// path, so "the values the steps used" are exactly the copy, and a line the L1 cached
-// before the wait cannot leak into the recompute.
+//     (cp.async.cg / ld.global.cg) and compared bitwise with the values the steps used.  On a
+//     difference every step of the instance is recomputed from the re-read values.
+// Before the wait, each thread stages its targets row in its slot of the CTA's shared memory
+// (ChainPdlSlot) with cp.async, so that every copy of the row is in flight at once and none
+// takes a register; the re-read goes to a second row of the same slot, in flight at once too.
+// The steps read the row from that slot, never through the read-only path, so "the values the
+// steps used" are exactly the slot, and a line the L1 cached before the wait cannot leak into
+// the recompute.
 // PK_CHAIN_PDL=0 (compile time) launches the plain instantiation only, for A/B runs.
 #ifndef PK_CHAIN_PDL
 #define PK_CHAIN_PDL 1
@@ -340,35 +343,74 @@ __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;"
 // flags bit: after the wait, recompute every instance as if its inputs had changed (tests)
 constexpr int kChainForceRecompute = 4;
 
-template <bool CG>
-__device__ __forceinline__ float4 chain_ld4(const float* p) {
-  if constexpr (CG) return __ldcg(reinterpret_cast<const float4*>(p));
-  else return __ldg(reinterpret_cast<const float4*>(p));
+// One thread's slot of the PDL instantiation's staging buffer, in words: [targets row | q row |
+// re-read targets row], each part starting on a 16-byte boundary and sized for the longest row
+// the instantiation accepts (chain_row_words), so that every offset is a compile-time constant.
+// The slot stride is 4 words times an odd number: the eight threads of each phase of a 128-bit
+// shared load hit eight distinct 16-byte bank groups.
+template <int NJ, int NFT>
+struct ChainPdlSlot {
+  static constexpr int kRow = (chain_row_words(NJ, NFT) + 3) & ~3;
+  static constexpr int kQ = kRow;
+  static constexpr int kReread = (kQ + NJ + 3) & ~3;
+  static constexpr int kWords = ((kReread + kRow) / 4) % 2 ? kReread + kRow : kReread + kRow + 4;
+  // this thread's slot in a CTA of at most 128 threads; %tid.x is read with a volatile move,
+  // so the address is formed where it is used instead of being held in a register across
+  // the steps
+  static __device__ __forceinline__ float* row() {
+    __shared__ __align__(16) float rows[128 * kWords];
+    unsigned tid;
+    asm volatile("mov.u32 %0, %%tid.x;" : "=r"(tid));
+    return rows + tid * kWords;
+  }
+};
+
+__device__ __forceinline__ void cp_async_cg16(float* dst, const float* src) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"((unsigned)__cvta_generic_to_shared(dst)),
+               "l"(__cvta_generic_to_global(src))
+               : "memory");
 }
-// Copy the first `n` words of the targets row `src` to `dst` (local memory); returns
-// whether every word was bitwise equal to what `dst` held.  CG: read from L2.
-template <bool CG>
-__device__ __forceinline__ bool chain_copy_row(float* dst, const float* src, int n, bool v4) {
-  unsigned diff = 0u;
+__device__ __forceinline__ void cp_async_ca4(float* dst, const float* src) {
+  asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"((unsigned)__cvta_generic_to_shared(dst)),
+               "l"(__cvta_generic_to_global(src))
+               : "memory");
+}
+__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
+
+// Issue the copies of the `n`-word targets row `src` into shared `dst`, all of them before any
+// completes.  v4: n is a multiple of 4 and src is 16-byte aligned (128-bit copies, L2 only);
+// otherwise one 4-byte copy per word.  Nothing past the row is read.
+__device__ __forceinline__ void chain_stage_row(float* dst, const float* src, int n, bool v4) {
   if (v4) {
 #pragma unroll 1
-    for (int k = 0; k < n; k += 4) {
-      const float4 t = chain_ld4<CG>(src + k);
-      diff |= (__float_as_uint(t.x) ^ __float_as_uint(dst[k])) | (__float_as_uint(t.y) ^ __float_as_uint(dst[k + 1])) |
-              (__float_as_uint(t.z) ^ __float_as_uint(dst[k + 2])) | (__float_as_uint(t.w) ^ __float_as_uint(dst[k + 3]));
-      dst[k] = t.x;
-      dst[k + 1] = t.y;
-      dst[k + 2] = t.z;
-      dst[k + 3] = t.w;
-    }
+    for (int k = 0; k < n; k += 4) cp_async_cg16(dst + k, src + k);
   } else {
 #pragma unroll 1
-    for (int k = 0; k < n; ++k) {
-      const float t = CG ? __ldcg(src + k) : __ldg(src + k);
-      diff |= __float_as_uint(t) ^ __float_as_uint(dst[k]);
-      dst[k] = t;
-    }
+    for (int k = 0; k < n; ++k) cp_async_ca4(dst + k, src + k);
   }
+}
+// The re-read after the wait: from L2 only (a line the L1 cached before the wait may be stale).
+// The 4-byte form has no L2-only cp.async, so it loads with ld.global.cg.
+__device__ __forceinline__ void chain_reread_row(float* dst, const float* src, int n, bool v4) {
+  if (v4) {
+#pragma unroll 1
+    for (int k = 0; k < n; k += 4) cp_async_cg16(dst + k, src + k);
+  } else {
+#pragma unroll 4
+    for (int k = 0; k < n; ++k) dst[k] = __ldcg(src + k);
+  }
+}
+// Whether the first `n` words of the shared rows a and b (16-byte aligned) are bitwise equal.
+__device__ __forceinline__ bool chain_rows_equal(const float* a, const float* b, int n) {
+  unsigned diff = 0u;
+  int k = 0;
+#pragma unroll 1
+  for (; k + 4 <= n; k += 4) {
+    const uint4 x = *reinterpret_cast<const uint4*>(a + k), y = *reinterpret_cast<const uint4*>(b + k);
+    diff |= (x.x ^ y.x) | (x.y ^ y.y) | (x.z ^ y.z) | (x.w ^ y.w);
+  }
+#pragma unroll 1
+  for (; k < n; ++k) diff |= __float_as_uint(a[k]) ^ __float_as_uint(b[k]);
   return diff == 0u;
 }
 
@@ -402,39 +444,43 @@ __global__ void __launch_bounds__(128, 4)
 #pragma unroll
     for (int k = 0; k < NJ; ++k) qi[k] = __ldg(qrow + k);
   }
-  const float* grow = targets + i * (int64_t)P.target_stride;
-  const float* trow = grow;
-  // PDL: [targets row (target_stride <= chain_row_words words) | q row] as the steps use them
-  __align__(16) float used[PDL ? chain_row_words(NJ, NFT) + NJ : 1];
-  float* const used_q = used + (PDL ? chain_row_words(NJ, NFT) : 0);
-  const bool v4 = P.target_vec4 && (reinterpret_cast<uintptr_t>(grow) & 15u) == 0u;
-  if constexpr (PDL) {
-    chain_copy_row<false>(used, grow, P.target_stride, v4);
-#pragma unroll
-    for (int k = 0; k < NJ; ++k) used_q[k] = qi[k];
-    trow = used;
-  }
+  const float* const grow = targets + i * (int64_t)P.target_stride;
   int st_all;
+  if constexpr (!PDL) {
+    st_all = rollout_chain<NJ, NFT, true>(P, qi, grow, vi, n_steps, q_out != nullptr, flags, T, B, i);
+  } else {
+    using L = ChainPdlSlot<NJ, NFT>;
+    const int n = P.target_stride;  // <= chain_row_words(NJ, NFT)
+    const bool v4 = (n & 3) == 0 && (reinterpret_cast<uintptr_t>(grow) & 15u) == 0u;
+    {
+      float* const row = L::row();
+      chain_stage_row(row, grow, n, v4);
+#pragma unroll
+      for (int k = 0; k < NJ; ++k) row[L::kQ + k] = qi[k];
+    }
+    cp_async_wait_all();  // each thread reads only its own slot: no barrier
+    PK_PHASE(kPhaseLoaded);
 #pragma unroll 1
-  for (int pass = 0;; ++pass) {
-    st_all = rollout_chain<NJ, NFT, !PDL>(P, qi, trow, vi, n_steps, q_out != nullptr, flags, T, B, i);
-    if constexpr (!PDL) {
-      break;
-    } else {
+    for (int pass = 0;; ++pass) {
+      st_all = rollout_chain<NJ, NFT, false>(P, qi, L::row() + (pass ? L::kReread : 0), vi, n_steps, q_out != nullptr,
+                                             flags, T, B, i);
       if (pass > 0) break;
       pdl_wait();
       // the inputs as the predecessors left them; one recompute at most (nothing writes
       // them once the predecessors are complete)
-      bool same = chain_copy_row<true>(used, grow, P.target_stride, v4) && !(flags & kChainForceRecompute);
+      float* const row = L::row();
+      chain_reread_row(row + L::kReread, grow, n, v4);
+      float qn[NJ];
+      bool same = !(flags & kChainForceRecompute);
 #pragma unroll
       for (int k = 0; k < NJ; ++k) {
-        const float t = __ldcg(qrow + k);
-        same &= __float_as_uint(t) == __float_as_uint(used_q[k]);
-        used_q[k] = t;
+        qn[k] = __ldcg(qrow + k);
+        same &= __float_as_uint(qn[k]) == __float_as_uint(row[L::kQ + k]);
       }
-      if (same) break;
+      cp_async_wait_all();
+      if (same && chain_rows_equal(row, row + L::kReread, n)) break;
 #pragma unroll
-      for (int k = 0; k < NJ; ++k) qi[k] = used_q[k];
+      for (int k = 0; k < NJ; ++k) qi[k] = qn[k];
     }
   }
   PK_PHASE(kPhaseWaited);
@@ -453,33 +499,35 @@ __global__ void __launch_bounds__(128, 4)
   // instruction writes 512 contiguous bytes per warp (full 128-byte lines on the wire) instead
   // of 8-byte pieces at a 4 NJ-byte stride (measured at N = 8: the strided form ran the link at
   // about a third of its rate).
-  if (peers.n > 0) {
-    __shared__ __align__(16) float stage[8][32 * NJ];
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int64_t row0 = i - lane;  // first row of this warp
-    const bool vec = (row0 + 32 <= B) && warp < 8 && ((peers.row_offset * NJ) % 4 == 0);
-    if (vec) {
-      float* st = stage[warp];
+  if constexpr (!PDL) {  // the PDL instantiation never runs with peers
+    if (peers.n > 0) {
+      __shared__ __align__(16) float stage[8][32 * NJ];
+      const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+      const int64_t row0 = i - lane;  // first row of this warp
+      const bool vec = (row0 + 32 <= B) && warp < 8 && ((peers.row_offset * NJ) % 4 == 0);
+      if (vec) {
+        float* st = stage[warp];
 #pragma unroll
-      for (int k = 0; k < NJ; ++k) st[lane * NJ + k] = vi[k];
-      __syncwarp();
-      constexpr int NV4 = 32 * NJ / 4;
-      // destinations in a per-rank, per-CTA rotated order: all ranks storing to peer 0 first,
-      // then peer 1, ... would converge on one NVSwitch port at a time
-      const int first = peers.rank + 1 + (int)(blockIdx.x % (unsigned)peers.n);
+        for (int k = 0; k < NJ; ++k) st[lane * NJ + k] = vi[k];
+        __syncwarp();
+        constexpr int NV4 = 32 * NJ / 4;
+        // destinations in a per-rank, per-CTA rotated order: all ranks storing to peer 0 first,
+        // then peer 1, ... would converge on one NVSwitch port at a time
+        const int first = peers.rank + 1 + (int)(blockIdx.x % (unsigned)peers.n);
 #pragma unroll 1
-      for (int t = 0; t < peers.n; ++t) {
-        const int p = (first + t) % peers.n;
-        float4* dst = reinterpret_cast<float4*>(peers.ptr[p] + (peers.row_offset + row0) * NJ);
+        for (int t = 0; t < peers.n; ++t) {
+          const int p = (first + t) % peers.n;
+          float4* dst = reinterpret_cast<float4*>(peers.ptr[p] + (peers.row_offset + row0) * NJ);
 #pragma unroll
-        for (int f = lane; f < NV4; f += 32) dst[f] = reinterpret_cast<const float4*>(st)[f];
-      }
-    } else {
+          for (int f = lane; f < NV4; f += 32) dst[f] = reinterpret_cast<const float4*>(st)[f];
+        }
+      } else {
 #pragma unroll 1
-      for (int p = 0; p < peers.n; ++p) {
-        float* prow = peers.ptr[p] + (peers.row_offset + i) * NJ;
+        for (int p = 0; p < peers.n; ++p) {
+          float* prow = peers.ptr[p] + (peers.row_offset + i) * NJ;
 #pragma unroll
-        for (int k = 0; k < NJ; ++k) prow[k] = vi[k];
+          for (int k = 0; k < NJ; ++k) prow[k] = vi[k];
+        }
       }
     }
   }

@@ -140,8 +140,7 @@ PK_HD T load_ro(const T* p) {
 PK_HD SE3f load_se3_vec4(const float* t, bool vec4) {
 #if defined(__CUDA_ARCH__)
   // the caller's `vec4` covers stride and offsets; the base pointer is checked here (a
-  // sliced tensor may start anywhere).  __ldg only reads global memory: a row the chain
-  // kernel copied to local memory takes the plain loads (resolved at compile time).
+  // sliced tensor may start anywhere).  __ldg only reads global memory.
   if (vec4 && __isGlobal(t) && (reinterpret_cast<uintptr_t>(t) & 15u) == 0u) {
     const float4 a = __ldg(reinterpret_cast<const float4*>(t));
     const float4 b = __ldg(reinterpret_cast<const float4*>(t) + 1);
@@ -150,6 +149,19 @@ PK_HD SE3f load_se3_vec4(const float* t, bool vec4) {
     T.R.m[0] = a.x; T.R.m[1] = a.y; T.R.m[2] = a.z; T.p.x = a.w;
     T.R.m[3] = b.x; T.R.m[4] = b.y; T.R.m[5] = b.z; T.p.y = b.w;
     T.R.m[6] = c.x; T.R.m[7] = c.y; T.R.m[8] = c.z; T.p.z = c.w;
+    return T;
+  }
+  // a row the PDL instantiation of the chain kernel staged in shared memory: 128-bit LDS
+  // (volatile: ordered after that kernel's cp.async.wait_all)
+  if (vec4 && __isShared(t) && (reinterpret_cast<uintptr_t>(t) & 15u) == 0u) {
+    const unsigned s = (unsigned)__cvta_generic_to_shared(t);
+    SE3f T;
+    asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];"
+        : "=f"(T.R.m[0]), "=f"(T.R.m[1]), "=f"(T.R.m[2]), "=f"(T.p.x) : "r"(s));
+    asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4+16];"
+        : "=f"(T.R.m[3]), "=f"(T.R.m[4]), "=f"(T.R.m[5]), "=f"(T.p.y) : "r"(s));
+    asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4+32];"
+        : "=f"(T.R.m[6]), "=f"(T.R.m[7]), "=f"(T.R.m[8]), "=f"(T.p.z) : "r"(s));
     return T;
   }
 #else
@@ -426,6 +438,7 @@ PK_HD bool step_failed(int st_all, int safety_break) {
 // (scripts/chain_phases.py).
 enum ChainPhase {
   kPhaseEntry = 0,     // kernel entry
+  kPhaseLoaded,        // q and the targets row have landed (PDL instantiation; 0 in the plain one)
   kPhaseAssembled,     // after ChainStep::assemble (limit check, FK, task rows, box)
   kPhaseCorner,        // after the corner test of BoxLSQChol::corner_start
   kPhaseClosedForm,    // after the closed-form releases (corner_start returned)

@@ -11,8 +11,8 @@ GPU mode compiles an instrumented copy of the library (__graft_entry__.NVCC_FLAG
 loads it in place of pink_b200/libpink_b200.so.  It runs the bench.py workload (UR5, same seed,
 B = 65536, 32 rotating input sets, PDL as the library launches it) as one CUDA graph of K
 launches, R times, and reads back after each the records of all its launches: for every
-warp the %globaltimer and clock64 values at kernel entry, after ChainStep::assemble, after the
-corner test of BoxLSQChol::corner_start, after the closed-form releases, after the rounds, after
+warp the %globaltimer and clock64 values at kernel entry, once q and the targets row have landed
+(before the first step), after ChainStep::assemble, after the corner test of BoxLSQChol::corner_start, after the closed-form releases, after the rounds, after
 griddepcontrol.wait and after the last store (pk_math.cuh, ChainPhase).  A mark holds the largest
 value over the warp's lanes, so a phase of a warp lasts until its slowest lane is through.  It
 prints, per phase, the median and p99 duration per warp, the span from the first warp's entry
@@ -41,14 +41,14 @@ sys.path.insert(0, ROOT)
 from __graft_entry__ import NVCC_FLAGS  # noqa: E402
 
 CSRC = os.path.join(ROOT, "pink_b200", "csrc")
-PHASES = ["entry", "assemble", "corner", "closed_form", "rounds", "wait", "store"]
+PHASES = ["entry", "loaded", "assemble", "corner", "closed_form", "rounds", "wait", "store"]
 FLAGS = {"release1": 1, "release2": 2, "rounds": 4}
 KERNEL = "ik_chain_kernel<6, 1, true>"
 MAX_WARPS = 65536  # pk::kChainPhaseMaxWarps
 
 
 class Record(C.Structure):  # pk::ChainPhaseRecord
-    _fields_ = [("ns", C.c_uint64 * 7), ("clk", C.c_uint64 * 7), ("smid", C.c_uint32), ("flags", C.c_uint32)]
+    _fields_ = [("ns", C.c_uint64 * len(PHASES)), ("clk", C.c_uint64 * len(PHASES)), ("smid", C.c_uint32), ("flags", C.c_uint32)]
 
 
 def build_instrumented(out_dir):
@@ -123,7 +123,7 @@ def gpu_phases(args):
     if args.steps * nw > MAX_WARPS:
         raise SystemExit(f"--steps {args.steps}: at most {MAX_WARPS // nw} launches of {nw} warps fit the records")
     buf = (Record * MAX_WARPS)()
-    dt = np.dtype([("ns", "<u8", 7), ("clk", "<u8", 7), ("smid", "<u4"), ("flags", "<u4")])
+    dt = np.dtype([("ns", "<u8", len(PHASES)), ("clk", "<u8", len(PHASES)), ("smid", "<u4"), ("flags", "<u4")])
     lib.pk_chain_phase_records(C.addressof(buf), MAX_WARPS, 4)  # drop the warm-up's records
     regions = []
     for _ in range(args.regions):
@@ -145,6 +145,7 @@ def report(regions, kname, B, args, gpu, bad):
     # every launch but the first of each replay, which has no predecessor to overlap
     rec = np.concatenate([r[1:].reshape(-1) for r in regions])
     ns, clk, flags = rec["ns"].astype(np.int64), rec["clk"].astype(np.int64), rec["flags"]
+    CF, RD = PHASES.index("closed_form"), PHASES.index("rounds")
     done = (ns > 0).all(axis=1)  # every warp passes every mark in this workload
     total_clk = clk[done, -1] - clk[done, 0]
     total_ns = ns[done, -1] - ns[done, 0]
@@ -161,19 +162,19 @@ def report(regions, kname, B, args, gpu, bad):
         d = (clk[:, k] - clk[:, k - 1]) / cyc_per_ns
         print(f"{PHASES[k - 1] + ' -> ' + PHASES[k]:<34}{np.median(d):>10.0f}{np.quantile(d, 0.99):>10.0f}"
               f"{d.mean():>10.0f}{np.median(d) / med_total:>22.1%}")
-    work = (clk[:, 4] - clk[:, 0]) / cyc_per_ns
-    common = (clk[:, 3] - clk[:, 0]) / cyc_per_ns
+    work = (clk[:, RD] - clk[:, 0]) / cyc_per_ns
+    common = (clk[:, CF] - clk[:, 0]) / cyc_per_ns
     print(f"{'entry -> store (whole warp)':<34}{med_total:>10.0f}{np.quantile(total_clk, 0.99) / cyc_per_ns:>10.0f}"
           f"{total_clk.mean() / cyc_per_ns:>10.0f}")
     print(f"{'entry -> rounds (before the wait)':<34}{np.median(work):>10.0f}{np.quantile(work, 0.99):>10.0f}"
           f"{work.mean():>10.0f}")
-    print(f"# entry -> closed_form (assemble + corner + releases), median warp: {np.median(common):.0f} ns = "
+    print(f"# entry -> closed_form (loads + assemble + corner + releases), median warp: {np.median(common):.0f} ns = "
           f"{np.median(common) / np.median(work):.1%} of the median entry -> rounds, "
           f"{np.median(common) / med_total:.1%} of the median entry -> store")
     only1 = (flags & 6) == 0
     if only1.any():
-        c1 = (clk[only1, 3] - clk[only1, 0]) / cyc_per_ns
-        w1 = (clk[only1, 4] - clk[only1, 0]) / cyc_per_ns
+        c1 = (clk[only1, CF] - clk[only1, 0]) / cyc_per_ns
+        w1 = (clk[only1, RD] - clk[only1, 0]) / cyc_per_ns
         print(f"# warps with no second release and no rounds ({only1.mean():.1%}): assemble + corner + first release "
               f"median {np.median(c1):.0f} ns of {np.median(w1):.0f} ns before the wait")
     spans, works, gaps = [], [], []
@@ -181,7 +182,7 @@ def report(regions, kname, B, args, gpu, bad):
         n = r["ns"].astype(np.int64)
         for k in range(1, n.shape[0]):
             spans.append(n[k, :, -1].max() - n[k, :, 0].min())
-            works.append(n[k, :, 4].max() - n[k, :, 0].min())
+            works.append(n[k, :, RD].max() - n[k, :, 0].min())
             gaps.append(n[k, :, -1].max() - n[k - 1, :, -1].max())
     print(f"# per launch (globaltimer): first warp entry -> last warp store median {np.median(spans):.0f} ns "
           f"(min {np.min(spans):.0f}, max {np.max(spans):.0f}); first entry -> last warp past the rounds median "
