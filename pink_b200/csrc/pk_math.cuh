@@ -371,22 +371,24 @@ PK_HD void integrate_configuration(int nq, int free_flyer, const float* qi,
     const V3 w = dt * v3(vi[3], vi[4], vi[5]);
     const float x = dot(w, w);
     const float th = sqrtf(x);
+    float sh, ch;  // sin, cos of th/2: the quaternion step, and b
+    sincos_f(0.5f * th, &sh, &ch);
     float b, c;  // (1 - cos)/th^2, (th - sin)/th^3
     if (th < 1e-2f) {
       b = 0.5f - x / 24.f + x * x / 720.f;
       c = 1.f / 6.f - x / 120.f + x * x / 5040.f;
     } else {
+      // b = (sin(th/2) / (th/2))^2 / 2: 1 - cos(th) would cancel to ~11 bits at th ~ 1e-2
+      const float r = sh / (0.5f * th);
+      b = 0.5f * r * r;
       float s, co;
       sincos_f(th, &s, &co);
-      b = (1.f - co) / x;
       c = (th - s) / (x * th);
     }
     const V3 wv = cross(w, vl);
     const V3 t = vl + b * wv + c * cross(w, wv);
     const V3 p = mul(R, t);
     o[0] = qi[0] + p.x; o[1] = qi[1] + p.y; o[2] = qi[2] + p.z;
-    float sh, ch;
-    sincos_f(0.5f * th, &sh, &ch);
     const float k = th < 1e-4f ? 0.5f : sh / th;
     const float dx = k * w.x, dy = k * w.y, dz = k * w.z, dw = ch;
     const float n0 = rsqrtf(qi[3] * qi[3] + qi[4] * qi[4] + qi[5] * qi[5] + qi[6] * qi[6]);
