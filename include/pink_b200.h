@@ -303,6 +303,25 @@ int pk_converge_multistart_prepared(const PkModel* model, const PkProblem* probl
                                     float* err, int32_t* seed, int32_t* steps, int32_t* status,
                                     int64_t B, void* stream);
 
+/* Gradient of a loss with respect to the targets at solutions of pk_converge_prepared /
+ * pk_converge_multistart_prepared: grad_targets[b] = (d q_star / d T)^T grad_q[b] at q_star[b]
+ * (targets[B][target_stride] the rows the solutions were converged to, grad_q[B][nq] the loss
+ * gradient in q coordinates).  The converge loop stops where the step's linear term vanishes on
+ * the coordinates it leaves off the configuration limits; the gradient is that condition's
+ * implicit derivative with the Gauss-Newton matrix N = sum_t alpha_t J_t^T W_t^2 J_t (DESIGN.md
+ * section 3.2f).  Coordinates held on a configuration limit do not move; a frame target's 12
+ * floats [R | p] receive [1/2 R [g_w]x | R g_v] from the gradient (g_v, g_w) of the twist d in
+ * T <- T exp(d); shared targets get nothing (their row entries stay 0).
+ *   status[B]  0, or PK_STATUS_NOT_POSDEF: N on the free coordinates is not positive definite
+ *              in fp32 (the row is 0); may be NULL.
+ * The caller zeroes the rows of instances that did not converge.  Problems with barriers,
+ * equality constraints or an AccelerationLimit are rejected.  One launch of the general
+ * path's kernel on every model; no host synchronisation and no allocation, so the call can
+ * be captured in a CUDA graph.                                                             */
+int pk_converge_vjp_prepared(const PkModel* model, const PkProblem* problem, const float* q_star,
+                             const float* targets, const float* grad_q, float* grad_targets,
+                             int32_t* status, int64_t B, void* stream);
+
 /* ---- multi-GPU: all-gather of v through NVLink peer memory (SURVEY.md section 8e) ----
  * One process per GPU; instances are independent, so the only exchange is the one
  * BASELINE north_star names: collecting v.  Instead of a collective after the kernel, the

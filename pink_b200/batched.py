@@ -39,7 +39,9 @@ class RolloutTrajectory(NamedTuple):
 class Convergence(NamedTuple):
     """Result of :meth:`BatchedIK.converge`: ``q [B, nq]`` where each instance stopped,
     ``error [B]`` its error there, ``steps [B]`` the solves that ran, ``status [B]`` the OR of
-    their statuses (0 if none ran), ``converged [B]`` = ``error <= tol``."""
+    their statuses (0 if none ran), ``converged [B]`` = ``error <= tol``.  When the call was made
+    with ``targets.requires_grad`` (and grad mode on), ``q`` carries the implicit gradient with
+    respect to ``targets`` (:meth:`BatchedIK.converge_vjp`); the other fields never do."""
 
     q: torch.Tensor
     error: torch.Tensor
@@ -52,7 +54,8 @@ class MultistartConvergence(NamedTuple):
     """Result of :meth:`BatchedIK.converge_multistart`, per target: ``q [B, nq]`` the winning
     seed's configuration, ``error [B]`` its error, ``seed [B]`` (int32) its index, ``steps [B]``
     the rounds the group ran, ``status [B]`` the OR of the winner's step statuses (0 if it ran
-    none), ``converged [B]`` = ``error <= tol``."""
+    none), ``converged [B]`` = ``error <= tol``.  ``q`` carries a gradient as in
+    :class:`Convergence`, through the winning seed."""
 
     q: torch.Tensor
     error: torch.Tensor
@@ -63,6 +66,23 @@ class MultistartConvergence(NamedTuple):
 
 
 SEED_COUNTS = (1, 2, 4, 8, 16, 32)
+
+
+class _SolutionOfTargets(torch.autograd.Function):
+    """``q*`` as a function of ``targets``: the backward is one :meth:`BatchedIK.converge_vjp`
+    launch, with the rows of instances that did not converge set to zero."""
+
+    @staticmethod
+    def forward(ctx, targets, solver, q_star, ok):
+        ctx.solver = solver
+        ctx.save_for_backward(targets, q_star, ok)
+        return q_star.view_as(q_star)
+
+    @staticmethod
+    def backward(ctx, grad_q):
+        targets, q_star, ok = ctx.saved_tensors
+        grad_targets, _ = ctx.solver.converge_vjp(q_star, targets.detach(), grad_q.float().contiguous())
+        return torch.where(ok[:, None], grad_targets, torch.zeros_like(grad_targets)), None, None, None
 
 
 class BatchedIK:
@@ -273,10 +293,17 @@ class BatchedIK:
 
         Poses resolve to about 1e-7 in fp32, so a ``tol`` below about 1e-6 may run to
         ``max_steps``.  Asynchronous on the current stream; no allocation inside the library,
-        so the call can be captured in a CUDA graph.  ``q_out`` may be ``q``."""
+        so the call can be captured in a CUDA graph.  ``q_out`` may be ``q``.
+
+        With ``targets.requires_grad`` (and grad mode on) the returned ``q`` carries the gradient
+        with respect to ``targets``, one :meth:`converge_vjp` launch in the backward pass, zero
+        for instances that did not converge.  Every frame, relative frame and CoM task must then
+        be in ``tasks`` (so that ``tol`` bounds the gradient's error), and problems with barriers,
+        constraints or ``AccelerationLimit`` are rejected (``ValueError``)."""
         eng = self.engine
         B = q.shape[0]
         mask, tol = self._stop_test(tasks, tol, max_steps)
+        grad = self._grad_mode(targets, mask)
         if tuple(q.shape) != (B, self.nq) or q.dtype != torch.float32 or not q.is_contiguous():
             raise ValueError(f"q must be a contiguous float32 [B, {self.nq}] tensor")
         self._check_fixed_targets(targets, B)
@@ -292,7 +319,86 @@ class BatchedIK:
             _cabi.check(eng.lib.pk_converge_prepared(eng.handle, self._handle, _addr(q), _addr(targets), mask, tol,
                                                      int(max_steps), _addr(q_out), _addr(error), _addr(steps),
                                                      _addr(status), B, _stream(eng.device)))
+        if grad:
+            q_out = _SolutionOfTargets.apply(targets, self, q_out, self._solved(error, status, tol))
         return Convergence(q_out, error, steps, status, error <= tol)
+
+    def converge_vjp(self, q_star: torch.Tensor, targets: Optional[torch.Tensor], grad_q: torch.Tensor,
+                     grad_targets: Optional[torch.Tensor] = None, status: Optional[torch.Tensor] = None):
+        """Gradient of a loss with respect to ``targets [B, target_stride]`` at solutions ``q_star
+        [B, nq]`` of :meth:`converge` / :meth:`converge_multistart`, given ``grad_q [B, nq]``, the
+        loss gradient with respect to ``q_star``: ``(grad_targets [B, target_stride], status
+        [B])``.  :meth:`converge` attaches the same computation to its ``q`` when ``targets``
+        requires grad.
+
+        The loop stops where the step's linear term ``c = sum_t alpha_t J_t^T W_t^2 e_t`` vanishes
+        on the coordinates it leaves off the configuration limits; the gradient is that
+        condition's implicit derivative, ``dq*/dT = -N_FF^-1 dc_F/dT``, with the Gauss-Newton
+        ``N = sum_t alpha_t J_t^T W_t^2 J_t``.  It does not depend on ``dt``, the damping or the
+        velocity limits, and it is exact up to terms proportional to the errors of the tasks at
+        ``q_star`` (bounded by ``tol`` when those tasks are in the stopping test).  Semantics:
+
+        * Only ``targets`` is differentiated: the gradient with respect to the start is zero (the
+          fixed point does not depend on it), and shared targets are constants.
+        * ``grad_q`` is in q coordinates; on a free-flyer root it is mapped to the tangent space
+          by the transpose of ``d(q (+) dq)/d dq`` at ``dq = 0`` (a quaternion component that only
+          changes the norm is dropped).
+        * A coordinate the step holds on a configuration limit does not move (``dq*_i = 0``).
+        * A frame target's 12 floats ``[R | p]`` receive ``[1/2 R [g_w]x | R g_v]``, with ``(g_v,
+          g_w)`` the gradient of the twist ``d`` in ``T <- T exp(d)``.  ``1/2 R [g_w]x`` is the
+          tangent component, so a rotation parameterisation upstream (quaternion, 6-D,
+          axis-angle) receives the exact gradient.  CoM, posture and joint-velocity targets are
+          differentiated coordinate-wise; the root coordinates of a free-flyer posture target get
+          zero.
+        * ``status``: 0, or ``PK_STATUS_NOT_POSDEF`` (4) where ``N_FF`` is not positive definite in
+          fp32 (for example a 7-joint arm with one frame task and no posture task); that row is
+          zero.  Rows of instances that did not converge are the caller's to discard
+          (the autograd path of :meth:`converge` zeroes them).
+
+        Problems with barriers, equality constraints or ``AccelerationLimit`` are rejected.
+        Asynchronous on the current stream; no allocation inside the library, so the call can be
+        captured in a CUDA graph."""
+        eng = self.engine
+        B = q_star.shape[0]
+        if tuple(q_star.shape) != (B, self.nq) or q_star.dtype != torch.float32 or not q_star.is_contiguous():
+            raise ValueError(f"q_star must be a contiguous float32 [B, {self.nq}] tensor")
+        if tuple(grad_q.shape) != (B, self.nq) or grad_q.dtype != torch.float32 or not grad_q.is_contiguous():
+            raise ValueError(f"grad_q must be a contiguous float32 [B, {self.nq}] tensor")
+        self._check_fixed_targets(targets, B)
+        if grad_targets is None:
+            grad_targets = torch.empty((B, self.target_stride), device=eng.device, dtype=torch.float32)
+        if status is None:
+            status = torch.empty((B,), device=eng.device, dtype=torch.int32)
+        with torch.cuda.device(eng.device):
+            _cabi.check(eng.lib.pk_converge_vjp_prepared(eng.handle, self._handle, _addr(q_star), _addr(targets),
+                                                         _addr(grad_q), _addr(grad_targets), _addr(status), B,
+                                                         _stream(eng.device)))
+        return grad_targets, status
+
+    def _grad_mode(self, targets: Optional[torch.Tensor], mask: int) -> bool:
+        """Whether :meth:`converge` / :meth:`converge_multistart` attach the gradient with respect
+        to ``targets``; checks that the problem is one whose gradient error ``tol`` bounds."""
+        if targets is None or not (torch.is_grad_enabled() and targets.requires_grad):
+            return False
+        for k in range(len(self.tasks)):
+            if int(self.prob.tasks[k].type) in (_cabi.PK_TASK_FRAME, _cabi.PK_TASK_RELATIVE_FRAME,
+                                                _cabi.PK_TASK_COM) and not (mask >> k) & 1:
+                raise ValueError(f"gradients of converge need every frame, relative frame and CoM task in the "
+                                 f"stopping test: {self.tasks[k]!r} is not in tasks")
+        if int(self.prob.nbarriers):
+            raise ValueError("gradients of converge do not support barriers")
+        if int(self.prob.nconstraints):
+            raise ValueError("gradients of converge do not support equality constraints")
+        if int(self.prob.acc_enabled):
+            raise ValueError("gradients of converge do not support AccelerationLimit")
+        return True
+
+    def _solved(self, error: torch.Tensor, status: torch.Tensor, tol: float) -> torch.Tensor:
+        """Instances whose gradient is kept: converged, with no failed step."""
+        failed = _cabi.PK_STATUS_NO_SOLUTION | _cabi.PK_STATUS_NOT_POSDEF
+        if int(self.prob.safety_break):
+            failed |= _cabi.PK_STATUS_OUT_OF_LIMITS
+        return (error <= tol) & ((status & failed) == 0)
 
     def _stop_test(self, tasks: Iterable, tol: float, max_steps: int):
         """The task mask and tol of :meth:`converge` / :meth:`converge_multistart`, validated."""
@@ -352,6 +458,7 @@ class BatchedIK:
         be captured in a CUDA graph.  ``q_seeds`` is only read and must not overlap ``q_out``."""
         eng = self.engine
         mask, tol = self._stop_test(tasks, tol, max_steps)
+        grad = self._grad_mode(targets, mask)
         if (q_seeds.dim() != 3 or q_seeds.shape[2] != self.nq or q_seeds.dtype != torch.float32
                 or not q_seeds.is_contiguous()):
             raise ValueError(f"q_seeds must be a contiguous float32 [B, S, {self.nq}] tensor")
@@ -379,6 +486,8 @@ class BatchedIK:
             _cabi.check(lib.pk_converge_multistart_prepared(
                 eng.handle, self._handle, _addr(q_seeds), S, _addr(targets), mask, tol, int(max_steps), _addr(q_out),
                 _addr(error), _addr(seed), _addr(steps), _addr(status), B, _stream(eng.device)))
+        if grad:
+            q_out = _SolutionOfTargets.apply(targets, self, q_out, self._solved(error, status, tol))
         return MultistartConvergence(q_out, error, seed, steps, status, error <= tol)
 
     def sample_seeds(self, q: torch.Tensor, num_seeds: int, generator: Optional[torch.Generator] = None) -> torch.Tensor:

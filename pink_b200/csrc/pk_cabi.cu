@@ -591,6 +591,19 @@ __global__ void __launch_bounds__(64)
   converge_generic_instance(G, M, P, q, targets, mask, tol, max_steps, q_out, err, steps, status, i);
 }
 
+// Gradient with respect to the targets at converged solutions (pk_converge_vjp_prepared), on every
+// model: solution_vjp_instance per thread.
+template <int NJMAX, int NVMAX>
+__global__ void __launch_bounds__(64)
+    ik_generic_solution_vjp_kernel(const DevModel M, const __grid_constant__ DevProblem P, const float* q_star,
+                                   const float* targets, const float* grad_q, float* grad_targets,
+                                   int32_t* __restrict__ status, int64_t B) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= B) return;
+  Generic<NJMAX, NVMAX> G;
+  solution_vjp_instance(G, M, P, q_star, targets, grad_q, grad_targets, status, i);
+}
+
 // Tree kernel: one instance per warp, per-instance state in the warp's slice of
 // dynamic shared memory (pk_tree.cuh).
 constexpr int kTreeWarpsPerBlock = 2;
@@ -826,6 +839,7 @@ struct PkProblem {
     else cudaFree(dev_ext);
   }
   pk::Selection sel;
+  std::string vjp_error;  // pk::check_vjp_problem: why pk_converge_vjp_prepared rejects the problem
   alignas(16) unsigned char chain_params[sizeof(pk::ChainParams<7>)];
   // parameter block of the sub-warp chain kernel's variant sel.lanes (the padding joints depend on it)
   alignas(16) unsigned char coop_params[sizeof(pk::CoopParams<8>)];
@@ -893,6 +907,7 @@ int prepare_problem(const PkModel* m, const PkProblemDesc* desc, PkProblem* pr, 
     return o;
   }();
   const pk::Selection& s = pr->sel = pk::select_kernel(m->hm, pr->P, hx, opts);
+  pr->vjp_error = pk::check_vjp_problem(hx);
   if (s.path != pk::kPathChain) return 0;
   const pk::DevExtras* X = hx.present ? &hx.X : nullptr;
   pk::with_chain(s, [&](auto nj, auto nft) {
@@ -1220,6 +1235,22 @@ extern "C" int pk_converge_multistart_prepared(const PkModel* m, const PkProblem
     return launch_rows(pk::ik_generic_multistart_kernel<decltype(nj)::value, decltype(nv)::value>, B * S, 64, stream,
                        m->dev, pr->P, q_seeds, S, targets, task_mask, tol, (int)max_steps, q_out, err, seed, steps,
                        status, B);
+  });
+}
+
+extern "C" int pk_converge_vjp_prepared(const PkModel* m, const PkProblem* pr, const float* q_star,
+                                        const float* targets, const float* grad_q, float* grad_targets,
+                                        int32_t* status, int64_t B, void* stream_) {
+  if (check_prepared(m, pr, q_star, targets, B, [&] {
+        if (!pr->vjp_error.empty()) return fail(pr->vjp_error);
+        if (B > 0 && !grad_q) return fail("null grad_q");
+        return B > 0 && pr->P.target_stride > 0 && !grad_targets ? fail("null grad_targets") : 0;
+      }))
+    return 1;
+  if (B == 0) return 0;
+  return pk::with_generic(pk::generic_size_class(m->hm), [&](auto nj, auto nv) {
+    return launch_rows(pk::ik_generic_solution_vjp_kernel<decltype(nj)::value, decltype(nv)::value>, B, 64,
+                       (cudaStream_t)stream_, m->dev, pr->P, q_star, targets, grad_q, grad_targets, status, B);
   });
 }
 

@@ -730,6 +730,170 @@ struct Generic {
     }
     if (out.status) *out.status = status;
   }
+
+  // Gradient of a loss with respect to the targets row at a converged solution q [nq]
+  // (pk_converge_vjp_prepared): gt [target_stride] = (dq*/dT)^T gq, gq [nq] the loss gradient with
+  // respect to q.  The converge loop stops moving where c_F(q, T) = 0, c = sum_t alpha_t J_t^T W_t^2
+  // e_t the step's linear term and F the coordinates its box QP leaves off the configuration limits
+  // (the held ones stay put: dq_i = 0); so dq*/dT = -N_FF^-1 dc_F/dT with the Gauss-Newton
+  // N = sum_t alpha_t J_t^T W_t^2 J_t (+ alpha w^2 on the posture diagonal), and
+  // gt = -(dc/dT)^T y, y = N_FF^-1 g_F, g the tangent gradient (DESIGN.md section 3.2f).  A frame
+  // target's 12 floats [R | p] receive [1/2 R [g_w]x | R g_v] from the twist gradient (g_v, g_w) of
+  // T <- T exp(d); shared targets get nothing.  Problems with barriers, constraints or an
+  // AccelerationLimit are rejected before this runs.  Returns 0, or PK_STATUS_NOT_POSDEF (gt = 0).
+  PK_HD int solution_vjp(const DevModel& M, const DevProblem& P, const float* q, const float* trow, const float* gq,
+                         float* gt) {
+    const int nv = M.nv;
+    const int rq = M.free_flyer ? 7 : 0;
+    const int rv = M.free_flyer ? 6 : 0;
+    for (int k = 0; k < P.target_stride; ++k) gt[k] = 0.f;
+    forward_kinematics(M, q);
+
+    // the step's QP at q (as step / finish build it), for its active set
+    float A[kGenericMaxRows][NVMAX];
+    float b[kGenericMaxRows], sa[kGenericMaxRows];  // sa: sqrt(alpha) of the row's task
+    float d[NVMAX], beta[NVMAX], pw2[NVMAX], pc[NVMAX], na2[NVMAX];
+    for (int i = 0; i < nv; ++i) { pw2[i] = 0.f; pc[i] = 0.f; na2[i] = 0.f; }
+    int K = 0;
+    float diag = P.damping;
+    float Jw[6][NVMAX];
+    for (int t = 0; t < P.ntasks; ++t) {
+      const DevTask& Kt = P.tasks[t];
+      const float* tgt = Kt.tgt_shared ? (P.shared + Kt.tgt_off) : (trow + Kt.tgt_off);
+      if (is_diag_task(Kt.type)) {
+        const float w2 = Kt.cost[0] * Kt.cost[0];
+        float se = 0.f;
+        for (int i = rv; i < nv; ++i) {
+          const float e = diag_task_error(Kt.type, q, tgt, i, rq, rv);
+          se = fmaf(e, e, se);
+          pw2[i] += w2;
+          pc[i] = fmaf(Kt.gain * w2, e, pc[i]);
+          if (Kt.type == PK_TASK_POSTURE) na2[i] = fmaf(Kt.gain, w2, na2[i]);
+        }
+        diag = fmaf(Kt.lm * Kt.gain * Kt.gain * w2, se, diag);
+        continue;
+      }
+      float e[6];
+      const int k = task_rows(M, P, Kt, q, tgt, e, Jw);
+      float mu = 0.f;
+      for (int r = 0; r < k; ++r) {
+        const float ew = Kt.cost[r] * Kt.gain * e[r];
+        mu = fmaf(ew, ew, mu);
+        if (Kt.cost[r] == 0.f) continue;
+        if (K < kGenericMaxRows) {
+          b[K] = ew;
+          sa[K] = sqrtf(Kt.gain);
+          for (int i = 0; i < nv; ++i) A[K][i] = Kt.cost[r] * Jw[r][i];
+        }
+        ++K;
+      }
+      diag = fmaf(Kt.lm, mu, diag);
+    }
+    if (K > kGenericMaxRows) return PK_STATUS_NOT_POSDEF;
+    float lo[NVMAX], hi[NVMAX];
+    uint64_t cfg_hi = 0ull, cfg_lo = 0ull;  // the configuration limit is the bound
+    for (int i = 0; i < nv; ++i) {
+      const float qi = (i >= rv) ? q[i + rq - rv] : 0.f;
+      const float vb = P.dt * P.vel[i];
+      const float ch = P.cfg_gain * (P.cfg_hi[i] - qi);
+      const float cl = P.cfg_gain * (P.cfg_lo[i] - qi);
+      hi[i] = fminf(ch, vb);
+      lo[i] = fmaxf(cl, -vb);
+      if (ch <= vb) cfg_hi |= 1ull << i;
+      if (cl >= -vb) cfg_lo |= 1ull << i;
+      const float dd = sqrtf(pw2[i] + diag);
+      d[i] = dd;
+      beta[i] = dd > 0.f ? pc[i] / dd : 0.f;
+    }
+    float x[NVMAX];
+    uint64_t active;
+    BoxLSQ<kGenericMaxRows, NVMAX>::run(A, b, d, beta, lo, hi, K, nv, x, &active);
+    uint64_t held = 0ull;
+    for (int i = 0; i < nv; ++i)
+      if (((active >> i) & 1ull) && (((x[i] == hi[i] ? cfg_hi : cfg_lo) >> i) & 1ull)) held |= 1ull << i;
+
+    // tangent gradient: the transpose of d(q (+) dq)/d dq at dq = 0
+    float g[NVMAX];
+    if (M.free_flyer) {
+      const V3 gv = mulT(quat_to_matrix(q[3], q[4], q[5], q[6]), v3(gq[0], gq[1], gq[2]));
+      // quaternion (x, y, z, w) <- (x, y, z, w) * (w_dq / 2, 1)
+      const V3 qv = v3(q[3], q[4], q[5]), gqv = v3(gq[3], gq[4], gq[5]);
+      const V3 gw = 0.5f * (q[6] * gqv + cross(gqv, qv) - gq[6] * qv);
+      g[0] = gv.x; g[1] = gv.y; g[2] = gv.z;
+      g[3] = gw.x; g[4] = gw.y; g[5] = gw.z;
+    }
+    for (int i = rv; i < nv; ++i) g[i] = gq[i + rq - rv];
+
+    // N = [diag(sqrt(na2)); sqrt(alpha) W J]^T [...]
+    for (int r = 0; r < K; ++r)
+      for (int i = 0; i < nv; ++i) A[r][i] *= sa[r];
+    for (int i = 0; i < nv; ++i) d[i] = sqrtf(na2[i]);
+    float y[NVMAX];
+    if (!BoxLSQ<kGenericMaxRows, NVMAX>::normal_solve(A, d, K, nv, held, g, y)) return PK_STATUS_NOT_POSDEF;
+
+    // gt = -(dc/dT)^T y, task by task; dc/dT = alpha J^T W^2 de/dT, so with w = alpha W^2 J y
+    // (row r: sqrt(alpha) cost_r (A_r . y)) a target's gradient is -(de/dT)^T w
+    int r0 = 0;
+    for (int t = 0; t < P.ntasks; ++t) {
+      const DevTask& Kt = P.tasks[t];
+      if (is_diag_task(Kt.type)) {
+        if (Kt.tgt_shared) continue;
+        // posture e = q - q*: -(-alpha w^2) y; joint velocity e = dq_ref: -(alpha w^2) y
+        const float s = (Kt.type == PK_TASK_POSTURE ? 1.f : -1.f) * Kt.gain * Kt.cost[0] * Kt.cost[0];
+        float* G = gt + Kt.tgt_off + (Kt.type == PK_TASK_POSTURE ? rq - rv : -rv);
+        for (int i = rv; i < nv; ++i) G[i] = fmaf(s, y[i], G[i]);
+        continue;
+      }
+      const int k = Kt.type == PK_TASK_LINEAR ? Kt.rows : Kt.type == PK_TASK_COM ? 3 : 6;
+      float w[6];
+      for (int r = 0; r < k; ++r) {
+        w[r] = 0.f;
+        if (Kt.cost[r] == 0.f) continue;
+        float s = 0.f;
+        for (int i = 0; i < nv; ++i) s = fmaf(A[r0][i], y[i], s);
+        w[r] = sa[r0] * Kt.cost[r] * s;
+        ++r0;
+      }
+      if (Kt.tgt_shared || Kt.type == PK_TASK_LINEAR) continue;
+      float* G = gt + Kt.tgt_off;
+      if (Kt.type == PK_TASK_COM) {
+        // e = com - com*
+        for (int r = 0; r < 3; ++r) G[r] += w[r];
+        continue;
+      }
+      const SE3f Tt = load_se3(trow + Kt.tgt_off);
+      const SE3f Tf = compose(body_placement(Kt.body), load_se3(M.fX + 12 * Kt.frame));
+      const V3 wl = v3(w[0], w[1], w[2]), wa = v3(w[3], w[4], w[5]);
+      M3 Am, Bm;
+      V3 gv, gw;  // twist gradient of T* <- T* exp(d)
+      if (Kt.type == PK_TASK_FRAME) {
+        // e = log6(T_bt), T_bt <- T_bt exp(d): de/dd = Jlog6(T_bt) = [A B; 0 A]
+        const SE3f Tbt = act_inv(Tf, Tt);
+        jlog6(Tbt, log3(Tbt.R), Am, Bm);
+        gv = -1.f * mulT(Am, wl);
+        gw = -1.f * (mulT(Bm, wl) + mulT(Am, wa));
+      } else {
+        // e = log6(T_tf), T_tf <- exp(-d) T_tf: de/dd = -Jlog6(T_tf) Ad_{T_tf^-1}
+        const SE3f Tr = compose(body_placement(Kt.root_body), load_se3(M.fX + 12 * Kt.root));
+        const SE3f Ttf = act_inv(Tt, act_inv(Tr, Tf));
+        jlog6(Ttf, log3(Ttf.R), Am, Bm);
+        const V3 zl = mul(Ttf.R, mulT(Am, wl));
+        gv = zl;
+        gw = cross(Ttf.p, zl) + mul(Ttf.R, mulT(Bm, wl) + mulT(Am, wa));
+      }
+      const V3 Gp = mul(Tt.R, gv);
+      const float hw[9] = {0.f, -gw.z, gw.y, gw.z, 0.f, -gw.x, -gw.y, gw.x, 0.f};
+      for (int a = 0; a < 3; ++a) {
+        for (int c2 = 0; c2 < 3; ++c2) {
+          float s = 0.f;
+          for (int m = 0; m < 3; ++m) s = fmaf(Tt.R.m[3 * a + m], hw[3 * m + c2], s);
+          G[4 * a + c2] = fmaf(0.5f, s, G[4 * a + c2]);
+        }
+      }
+      G[3] += Gp.x; G[7] += Gp.y; G[11] += Gp.z;
+    }
+    return 0;
+  }
 };
 
 // Solve to a tolerance (pk_converge_prepared), one instance on the general path; the loop of
@@ -822,6 +986,19 @@ PK_HD void converge_generic_instance(Generic<NJMAX, NVMAX>& G, const DevModel& M
                    e, n, st);
   if (err) err[i] = e;
   if (steps) steps[i] = n;
+  if (status) status[i] = st;
+}
+
+// Instance i of ik_generic_solution_vjp_kernel: Generic::solution_vjp on row i of q_star, targets,
+// grad_q and grad_targets, then the status (unless null).
+template <int NJMAX, int NVMAX>
+PK_HD void solution_vjp_instance(Generic<NJMAX, NVMAX>& G, const DevModel& M, const DevProblem& P,
+                                 const float* __restrict__ q_star, const float* __restrict__ targets,
+                                 const float* __restrict__ grad_q, float* __restrict__ grad_targets,
+                                 int32_t* __restrict__ status, int64_t i) {
+  const int64_t S = P.target_stride;
+  const int st = G.solution_vjp(M, P, q_star + i * M.nq, targets ? targets + i * S : nullptr, grad_q + i * M.nq,
+                                grad_targets ? grad_targets + i * S : nullptr);
   if (status) status[i] = st;
 }
 

@@ -112,9 +112,12 @@ struct BoxLSQ {
     return ok;
   }
 
-  // Returns status bits (0, NOT_POSDEF, NO_SOLUTION, ITER_LIMIT).
+  // Returns status bits (0, NOT_POSDEF, NO_SOLUTION, ITER_LIMIT).  `active` (unless null): the
+  // coordinates the solution holds on a bound (x_i is then exactly lo_i or hi_i).
   static PK_HD int run(const float (&A)[KA][N], const float (&b)[KA], const float (&d)[N], const float (&beta)[N],
-                       const float (&lo)[N], const float (&hi)[N], int K, int n, float (&x)[N]) {
+                       const float (&lo)[N], const float (&hi)[N], int K, int n, float (&x)[N],
+                       uint64_t* active = nullptr) {
+    if (active) *active = 0ull;
     int status = 0;
     // infeasible box <=> quadprog reports no solution
     for (int i = 0; i < n; ++i) {
@@ -212,7 +215,62 @@ struct BoxLSQ {
       at_hi &= ~drop;
       at_lo &= ~drop;
     }
+    if (active) *active = at_hi | at_lo;
     return status;
+  }
+
+  // y_F = (A_F^T A_F + diag(d_F)^2)^-1 g_F on the free coordinates F (bit i of `held` clear), y_i = 0
+  // on the held ones.  Householder QR of [diag(d); A] on the compacted free columns as in eqp, so the
+  // normal matrix is never formed in fp32; then R^T z = g_F and R y_F = z.  Returns false (y = 0) when
+  // a pivot of R is at most 1e-5 of its column's norm: the matrix is not positive definite to fp32
+  // accuracy.
+  static PK_HD bool normal_solve(const float (&A)[KA][N], const float (&d)[N], int K, int n, uint64_t held,
+                                 const float (&g)[N], float (&y)[N]) {
+    float Aw[KA][N];
+    float Rd[N], Ru[NU], z[N];
+    int idx[N];
+    int nf = 0;
+    for (int j = 0; j < n; ++j) {
+      y[j] = 0.f;
+      if (!((held >> j) & 1ull)) idx[nf++] = j;
+    }
+    for (int r = 0; r < K; ++r)
+      for (int c = 0; c < nf; ++c) Aw[r][c] = A[r][idx[c]];
+    bool ok = true;
+    for (int k = 0; k < nf; ++k) {
+      float sigma = 0.f;
+      for (int r = 0; r < K; ++r) sigma = fmaf(Aw[r][k], Aw[r][k], sigma);
+      const float alpha = d[idx[k]];
+      const float norm = sqrtf(fmaf(alpha, alpha, sigma));
+      const float v0 = alpha + norm;
+      const float tau = (sigma > 0.f) ? 1.f / (norm * v0) : 0.f;
+      Rd[k] = (sigma > 0.f) ? -norm : alpha;
+      for (int j = k + 1; j < nf; ++j) {
+        float s = 0.f;
+        for (int r = 0; r < K; ++r) s = fmaf(Aw[r][k], Aw[r][j], s);
+        s *= tau;
+        Ru[ut(k, j)] = -s * v0;
+        for (int r = 0; r < K; ++r) Aw[r][j] = fmaf(-s, Aw[r][k], Aw[r][j]);
+      }
+      // norm of the original column k
+      float c2 = alpha * alpha;
+      for (int r = 0; r < K; ++r) c2 = fmaf(A[r][idx[k]], A[r][idx[k]], c2);
+      ok = ok && fabsf(Rd[k]) > 1e-5f * sqrtf(c2);
+    }
+    if (!ok) return false;
+    for (int k = 0; k < nf; ++k) {
+      float s = g[idx[k]];
+      for (int j = 0; j < k; ++j) s = fmaf(-Ru[ut(j, k)], z[j], s);
+      z[k] = s / Rd[k];
+    }
+    for (int kk = 0; kk < nf; ++kk) {
+      const int k = nf - 1 - kk;
+      float s = z[k];
+      for (int j = k + 1; j < nf; ++j) s = fmaf(-Ru[ut(k, j)], z[j], s);
+      z[k] = s / Rd[k];
+      y[idx[k]] = z[k];
+    }
+    return true;
   }
 };
 

@@ -115,6 +115,17 @@ inline std::string check_multistart_seeds(const Selection& sel, int S) {
   return "";
 }
 
+// Problems pk_converge_vjp_prepared differentiates: tasks, the box limits and FloatingBaseVelocityLimit
+// (velocity bounds cannot be active at a fixed point); "" when supported.  Barriers, equality
+// constraints and AccelerationLimit would need rows of the KKT system the gradient does not carry.
+inline std::string check_vjp_problem(const HostExtras& hx) {
+  if (!hx.present) return "";
+  if (hx.X.nbarriers) return "gradients of converge do not support barriers";
+  if (hx.X.nconstraints) return "gradients of converge do not support equality constraints";
+  if (hx.X.acc_enabled) return "gradients of converge do not support AccelerationLimit";
+  return "";
+}
+
 // f(std::integral_constant<int, N>) for the run-time value: the chain kernels' joint count
 // (2..7, chain_eligible), frame-task count (0..2), sub-warp lanes (a coop_has_variant), the
 // general path's <NJMAX, NVMAX>.
