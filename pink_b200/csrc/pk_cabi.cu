@@ -333,6 +333,12 @@ __device__ __forceinline__ void peer_count_kernel(const PeerOut& peers) {
 // The steps read the row from that slot, never through the read-only path, so "the values the
 // steps used" are exactly the slot, and a line the L1 cached before the wait cannot leak into
 // the recompute.
+// Right after the trigger, CTAs 0 .. l2_ctas - 1 prefetch the whole grid's q and targets rows into
+// L2 (pk::chain_l2_prefetch_ctas).  Under PDL those CTAs start early, in the slots the previous
+// grid leaves free, while the rest of the grid starts together once the previous one retires;
+// the prefetch lets that burst load from L2 instead of HBM.  It fills L2 only, the point of
+// coherence: a predecessor's later write replaces the line there and the post-wait re-read (from
+// L2) sees it, so a line prefetched before that write cannot reach the results.
 // PK_CHAIN_PDL=0 (compile time) launches the plain instantiation only, for A/B runs.
 #ifndef PK_CHAIN_PDL
 #define PK_CHAIN_PDL 1
@@ -414,6 +420,23 @@ __device__ __forceinline__ bool chain_rows_equal(const float* a, const float* b,
   return diff == 0u;
 }
 
+// L2 prefetch of the floats [base, base + n) by the threads of CTAs 0 .. nctas - 1, each its own
+// slice of whole 16-byte groups of the range's 16-byte-aligned interior; the ragged ends are left
+// to the loads.  A hint: nothing is waited for, and no byte outside the range is addressed.
+__device__ __forceinline__ void chain_l2_prefetch(const float* base, int64_t n, int nctas) {
+  const uintptr_t a0 = (reinterpret_cast<uintptr_t>(base) + 15u) & ~uintptr_t(15);
+  const uintptr_t a1 = reinterpret_cast<uintptr_t>(base + n) & ~uintptr_t(15);
+  if (a1 <= a0) return;
+  const int64_t groups = (int64_t)((a1 - a0) >> 4), parts = (int64_t)nctas * blockDim.x;
+  const int64_t part = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const int64_t g0 = groups * part / parts, g1 = groups * (part + 1) / parts;
+  // one bulk prefetch per thread: faster on the benchmark than one prefetch.global.L2 per
+  // 128-byte line (DESIGN §3.1)
+  if (g1 > g0)
+    asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(a0 + 16 * (uintptr_t)g0),
+                 "r"((unsigned)(16 * (g1 - g0))));
+}
+
 // T: per-step targets and records of a trajectory call, read by the plain instantiation only.
 // The PDL protocol validates one copied targets row after the wait and stores nothing before
 // it, so it cannot cover K rows or per-step stores: trajectory calls with a step stride or
@@ -425,9 +448,15 @@ __global__ void __launch_bounds__(128, 4)
     ik_chain_kernel(const __grid_constant__ ChainParams<NJ> P, const float* __restrict__ q,
                     const float* __restrict__ targets, float* __restrict__ v, int32_t* __restrict__ status,
                     int64_t B, int flags, int n_steps, float* __restrict__ q_out,
-                    const __grid_constant__ PeerOut peers, const __grid_constant__ Trajectory T) {
+                    const __grid_constant__ PeerOut peers, const __grid_constant__ Trajectory T, int l2_ctas) {
   PK_PHASE(kPhaseEntry);
-  if constexpr (PDL) pdl_launch_dependents();
+  if constexpr (PDL) {
+    pdl_launch_dependents();
+    if (blockIdx.x < (unsigned)l2_ctas) {
+      chain_l2_prefetch(q, B * NJ, l2_ctas);
+      chain_l2_prefetch(targets, B * (int64_t)P.target_stride, l2_ctas);
+    }
+  }
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   peer_gate(peers);
   if (i >= B) return;
@@ -747,6 +776,38 @@ int launch_rows(void (*kernel)(Params...), int64_t rows, int block, cudaStream_t
 // a call the PDL instantiation of the chain kernel cannot run: per-step targets rows or records
 bool per_step(const pk::Trajectory& T) { return T.target_step != 0 || T.q || T.v || T.status; }
 
+// CTAs of the PDL chain kernel `kernel` the device holds at once at `block` threads, and its L2
+// size in bytes, queried once per device ordinal.  Zero when a query fails: no prefetch.
+struct ChainResidency {
+  std::mutex mu;
+  int64_t ctas[64] = {}, l2[64] = {};
+};
+template <class Kernel>
+void chain_residency(ChainResidency& r, Kernel kernel, int block, int64_t* ctas, int64_t* l2) {
+  int dev = 0;
+  *ctas = *l2 = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess) return;
+  std::lock_guard<std::mutex> lock(r.mu);
+  if (dev >= 0 && dev < 64 && r.ctas[dev] > 0) {
+    *ctas = r.ctas[dev];
+    *l2 = r.l2[dev];
+    return;
+  }
+  int per_sm = 0, sms = 0, l2_bytes = 0;
+  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, block, 0) != cudaSuccess ||
+      cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess ||
+      cudaDeviceGetAttribute(&l2_bytes, cudaDevAttrL2CacheSize, dev) != cudaSuccess) {
+    cudaGetLastError();
+    return;
+  }
+  *ctas = (int64_t)per_sm * sms;
+  *l2 = l2_bytes;
+  if (dev >= 0 && dev < 64) {
+    r.ctas[dev] = *ctas;
+    r.l2[dev] = *l2;
+  }
+}
+
 template <int NJ, int NFT>
 int launch_chain(const pk::ChainParams<NJ>& C, bool pdl_row_fits, const float* q, const float* targets, float* v,
                  int32_t* status, int64_t B, cudaStream_t stream, int n_steps, float* q_out, const pk::PeerOut& peers,
@@ -755,6 +816,8 @@ int launch_chain(const pk::ChainParams<NJ>& C, bool pdl_row_fits, const float* q
   static const int flags = (env_int("PK_CLOSED_FORM", 1) ? 0 : 1) | (env_int("PK_PROBE_SKIP_ROUNDS", 0) ? 2 : 0) |
                            (env_int("PK_CHAIN_FORCE_RECOMPUTE", 0) ? pk::kChainForceRecompute : 0);
   static const int block = env_int("PK_CHAIN_BLOCK", 128);
+  static const bool l2_prefetch = env_int("PK_CHAIN_L2_PREFETCH", 1) != 0;
+  static ChainResidency residency;
   const int64_t grid = (B + block - 1) / block;
   // PDL unless the fused peer gather is on (peer_gate and its flag protocol assume full stream
   // order), the targets row is longer than the kernel's copy of it, or a trajectory call reads
@@ -770,15 +833,21 @@ int launch_chain(const pk::ChainParams<NJ>& C, bool pdl_row_fits, const float* q
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr;
     cfg.numAttrs = 1;
+    int l2_ctas = 0;
+    if (l2_prefetch) {
+      int64_t resident, l2;
+      chain_residency(residency, pk::ik_chain_kernel<NJ, NFT, true>, block, &resident, &l2);
+      l2_ctas = pk::chain_l2_prefetch_ctas(grid, resident, B * 4 * (NJ + (int64_t)C.target_stride), l2);
+    }
     if (cudaLaunchKernelEx(&cfg, pk::ik_chain_kernel<NJ, NFT, true>, C, q, targets, v, status, B, flags, n_steps, q_out,
-                           peers, traj) == cudaSuccess)
+                           peers, traj, l2_ctas) == cudaSuccess)
       return launched();
     // a driver or capture mode that rejects the attribute: plain launches from now on
     cudaGetLastError();
     g_chain_pdl_rejected.store(true, std::memory_order_relaxed);
   }
   pk::ik_chain_kernel<NJ, NFT, false><<<(unsigned)grid, block, 0, stream>>>(C, q, targets, v, status, B, flags, n_steps,
-                                                                          q_out, peers, traj);
+                                                                          q_out, peers, traj, 0);
   return launched();
 }
 

@@ -433,8 +433,8 @@ PK_HD bool step_failed(int st_all, int safety_break) {
 // Phase clocks of the chain kernel (compile-time switch PK_CHAIN_PHASE_CLOCKS, off in the
 // product build, where PK_PHASE / PK_PHASE_FLAG expand to nothing).  Every warp keeps one
 // record: %globaltimer (ns) and clock64 at each phase boundary, the largest value over its
-// lanes (lanes that leave a stage early pass the next mark first), the SM it ran on and the
-// stages at least one of its lanes entered.  CTAs take consecutive record slots in the order
+// lanes (lanes that leave a stage early pass the next mark first), the SM it ran on, its CTA's
+// blockIdx.x and the stages at least one of its lanes entered.  CTAs take consecutive record slots in the order
 // they start, so the records of consecutive launches (which overlap under PDL) never share a
 // slot and come out grouped by launch.  Read back and reset by pk_chain_phase_records
 // (scripts/chain_phases.py).
@@ -454,6 +454,7 @@ struct ChainPhaseRecord {
   unsigned long long ns[kPhaseCount];
   unsigned long long clk[kPhaseCount];
   unsigned smid, flags;
+  unsigned cta, pad;  // blockIdx.x
 };
 constexpr int kChainPhaseMaxWarps = 65536;
 #if defined(PK_CHAIN_PHASE_CLOCKS) && defined(__CUDACC__)
@@ -489,6 +490,7 @@ __device__ __forceinline__ void chain_phase_mark(int k) {
     r->clk[0] = clk;
     r->smid = sm;
     r->flags = 0u;
+    r->cta = blockIdx.x;
     __threadfence_block();
   } else {
     atomicMax(&r->ns[k], ns);

@@ -3,7 +3,9 @@
 // run-time shape to the compile-time one.  Plain C++, no CUDA calls.
 #pragma once
 
+#include <algorithm>
 #include <cassert>
+#include <cstdint>
 #include <type_traits>
 
 #include "pk_marshal.hpp"
@@ -54,6 +56,22 @@ inline Selection select_kernel(const HostModel& m, const DevProblem& P, const Ho
     s.pdl_row_fits = P.target_stride <= chain_row_words(s.nj, s.nft);
   }
   return s;
+}
+
+// CTAs of a launch of the PDL chain kernel (ik_chain_kernel<NJ, NFT, true>) that prefetch the
+// whole grid's q and targets rows into L2 before their own loads; 0: no prefetch.  Under PDL the
+// next grid's lowest-index CTAs take the slots this grid leaves free and sit there until their
+// griddepcontrol.wait, while the rest of that grid starts together once this one retires; the
+// prefetch lets that burst load from L2 instead of HBM.  `resident`: CTAs the device holds at
+// once (occupancy per SM times the SM count).  Off when the grid is more than one wave (its
+// later CTAs start as earlier ones end, not together) or when the inputs take more than a
+// quarter of the L2 (they would evict one another, and whatever the running grid uses, before
+// the burst reads them).  Otherwise one CTA per slot left free, at least one, at most 32 and at
+// most the grid.
+constexpr int kChainL2PrefetchMaxCtas = 32;
+inline int chain_l2_prefetch_ctas(int64_t grid, int64_t resident, int64_t input_bytes, int64_t l2_bytes) {
+  if (grid <= 0 || grid > resident || input_bytes > l2_bytes / 4) return 0;
+  return (int)std::min<int64_t>({std::max<int64_t>(resident - grid, 1), kChainL2PrefetchMaxCtas, grid});
 }
 
 // A task mask of pk_converge_prepared (bit t: P.tasks[t]) in the chain kernels' slots: the frame

@@ -16,7 +16,10 @@ warp the %globaltimer and clock64 values at kernel entry, once q and the targets
 griddepcontrol.wait and after the last store (pk_math.cuh, ChainPhase).  A mark holds the largest
 value over the warp's lanes, so a phase of a warp lasts until its slowest lane is through.  It
 prints, per phase, the median and p99 duration per warp, the span from the first warp's entry
-to the last warp's end, and the share of warps in which at least one lane enters each stage.
+to the last warp's end, the share of warps in which at least one lane enters each stage, and
+the CTAs that entered well before their launch's median CTA (--early-ns): how many per launch,
+their blockIdx.x, their lead, how long they wait, and the load phase of those CTAs against the
+rest of the launch.
 
 --sass attributes every SASS instruction of ik_chain_kernel<6, 1, true> to a phase by the
 outermost source line of its inlining chain (nvdisasm -gi on a -lineinfo build).  --paths runs
@@ -48,7 +51,8 @@ MAX_WARPS = 65536  # pk::kChainPhaseMaxWarps
 
 
 class Record(C.Structure):  # pk::ChainPhaseRecord
-    _fields_ = [("ns", C.c_uint64 * len(PHASES)), ("clk", C.c_uint64 * len(PHASES)), ("smid", C.c_uint32), ("flags", C.c_uint32)]
+    _fields_ = [("ns", C.c_uint64 * len(PHASES)), ("clk", C.c_uint64 * len(PHASES)), ("smid", C.c_uint32),
+                ("flags", C.c_uint32), ("cta", C.c_uint32), ("pad", C.c_uint32)]
 
 
 def build_instrumented(out_dir):
@@ -123,7 +127,8 @@ def gpu_phases(args):
     if args.steps * nw > MAX_WARPS:
         raise SystemExit(f"--steps {args.steps}: at most {MAX_WARPS // nw} launches of {nw} warps fit the records")
     buf = (Record * MAX_WARPS)()
-    dt = np.dtype([("ns", "<u8", len(PHASES)), ("clk", "<u8", len(PHASES)), ("smid", "<u4"), ("flags", "<u4")])
+    dt = np.dtype([("ns", "<u8", len(PHASES)), ("clk", "<u8", len(PHASES)), ("smid", "<u4"), ("flags", "<u4"),
+                   ("cta", "<u4"), ("pad", "<u4")])
     lib.pk_chain_phase_records(C.addressof(buf), MAX_WARPS, 4)  # drop the warm-up's records
     regions = []
     for _ in range(args.regions):
@@ -189,6 +194,47 @@ def report(regions, kname, B, args, gpu, bad):
           f"{np.median(works):.0f} ns; last store of the previous launch -> last store median {np.median(gaps):.0f} ns")
     for name, bit in FLAGS.items():
         print(f"# warps with at least one lane in {name:<9}: {np.mean((flags & bit) != 0):.1%}")
+    early_ctas(regions, cyc_per_ns, args.early_ns)
+
+
+def early_ctas(regions, cyc_per_ns, lead_ns):
+    """CTAs that entered at least `lead_ns` before their launch's median CTA entry: how many per
+    launch, which blockIdx.x, how far ahead and how long their warps wait at griddepcontrol.wait;
+    and the load phase of the early CTAs against the rest (the burst)."""
+    LD, RD, WT = PHASES.index("loaded"), PHASES.index("rounds"), PHASES.index("wait")
+    counts, lowest, blocks, leads, waits, ld_early, ld_burst = [], [], [], [], [], [], []
+    for r in regions:
+        for k in range(1, r.shape[0]):
+            rec = r[k]
+            cta = rec["cta"].astype(np.int64)
+            ns, clk = rec["ns"].astype(np.int64), rec["clk"].astype(np.int64)
+            n = int(cta.max()) + 1
+            entry = np.full(n, np.iinfo(np.int64).max)
+            np.minimum.at(entry, cta, ns[:, 0])
+            lead = np.median(entry) - entry  # ns ahead of the median CTA entry
+            early = np.flatnonzero(lead >= lead_ns)
+            counts.append(len(early))
+            lowest.append(len(early) == 0 or int(early.max()) == len(early) - 1)
+            blocks.extend(early.tolist())
+            leads.extend(lead[early].tolist())
+            w_early = np.isin(cta, early)
+            waits.extend(((clk[w_early, WT] - clk[w_early, RD]) / cyc_per_ns).tolist())
+            ld = (clk[:, LD] - clk[:, 0]) / cyc_per_ns
+            ld_early.extend(ld[w_early].tolist())
+            ld_burst.extend(ld[~w_early].tolist())
+    counts = np.array(counts)
+    print(f"# early CTAs (entry >= {lead_ns / 1e3:g} us before the launch's median CTA entry): per launch median "
+          f"{np.median(counts):.0f} (min {counts.min()}, max {counts.max()}) over {len(counts)} launches; "
+          f"launches whose early CTAs are exactly blockIdx.x 0 .. count - 1: {np.mean(lowest):.1%}")
+    if not blocks:
+        return
+    b = np.array(blocks)
+    print(f"# early CTAs' blockIdx.x: min {b.min()}, median {np.median(b):.0f}, max {b.max()}; lead over the median "
+          f"entry median {np.median(leads):.0f} ns (min {np.min(leads):.0f}, max {np.max(leads):.0f}); their warps' "
+          f"rounds -> wait median {np.median(waits):.0f} ns (p99 {np.quantile(waits, 0.99):.0f})")
+    print(f"# entry -> loaded, median warp: early CTAs {np.median(ld_early):.0f} ns (p99 "
+          f"{np.quantile(ld_early, 0.99):.0f}), the other CTAs {np.median(ld_burst):.0f} ns (p99 "
+          f"{np.quantile(ld_burst, 0.99):.0f})")
 
 
 # ---- SASS per phase ---------------------------------------------------------------------------
@@ -326,6 +372,8 @@ def main():
     ap.add_argument("--steps", type=int, default=20, help="launches per CUDA graph")
     ap.add_argument("--regions", type=int, default=20, help="graph replays; the last launch of each is recorded")
     ap.add_argument("--batch", type=int, default=65536)
+    ap.add_argument("--early-ns", type=float, default=2000.0,
+                    help="a CTA entering at least this long before its launch's median CTA entry is early")
     ap.add_argument("--src", help="--sass: pink_b200/csrc the library was built from (default: the tree's)")
     ap.add_argument("--sass", action="store_true")
     ap.add_argument("--paths", action="store_true")
