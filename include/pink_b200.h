@@ -303,6 +303,29 @@ int pk_converge_multistart_prepared(const PkModel* model, const PkProblem* probl
                                     float* err, int32_t* seed, int32_t* steps, int32_t* status,
                                     int64_t B, void* stream);
 
+/* Goal-set solve to a tolerance: instance b is solved toward any of num_goals = G targets rows
+ * (goals) from num_seeds = S seeds, in one launch.  q_seeds[B*S][nq] as in
+ * pk_converge_multistart_prepared (every goal uses the same seeds); targets[B*G][target_stride]
+ * holds G complete rows per instance, goal g of instance b at row b*G + g.  The G*S members of
+ * an instance, j = g*S + s (goal-major, starting at q_seeds[b*S + s] toward goal g), form one
+ * group of pk_converge_multistart_prepared's rule: lockstep rounds, the group stops when one
+ * member has err <= tol, at max_steps, or when every member has failed, and the winner is the
+ * member with the smallest error at the stopping round (NaN counts as +inf, ties go to the
+ * lowest j: the earlier goal, then the earlier seed).  Per instance:
+ *   q_out[B][nq]  the winner's configuration (required; must not overlap q_seeds),
+ *   err[B]        its error, goal[B] = j / S, seed[B] = j % S, steps[B] the rounds the group
+ *                 ran, status[B] the OR of the winner's step statuses; all but q_out may be NULL.
+ * G and S are powers of two with G*S in {1, 2, 4, 8, 16, 32}; on the tree kernel G*S <= 8 and
+ * the G*S warp workspaces must fit one CTA's shared memory.  A goal count that is not a power
+ * of two is padded by repeating a goal: a duplicate never changes the winner.  G = 1 is
+ * pk_converge_multistart_prepared.  One launch, no host synchronisation and no allocation, so
+ * the call can be captured in a CUDA graph.                                                 */
+int pk_converge_goalset_prepared(const PkModel* model, const PkProblem* problem, const float* q_seeds,
+                                 int32_t num_seeds, const float* targets, int32_t num_goals,
+                                 uint32_t task_mask, float tol, int32_t max_steps, float* q_out,
+                                 float* err, int32_t* goal, int32_t* seed, int32_t* steps,
+                                 int32_t* status, int64_t B, void* stream);
+
 /* Gradient of a loss with respect to the targets at solutions of pk_converge_prepared /
  * pk_converge_multistart_prepared: grad_targets[b] = (d q_star / d T)^T grad_q[b] at q_star[b]
  * (targets[B][target_stride] the rows the solutions were converged to, grad_q[B][nq] the loss

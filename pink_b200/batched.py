@@ -65,6 +65,23 @@ class MultistartConvergence(NamedTuple):
     converged: torch.Tensor
 
 
+class GoalsetConvergence(NamedTuple):
+    """Result of :meth:`BatchedIK.converge_goalset`, per instance: ``q [B, nq]`` the winning
+    member's configuration, ``error [B]`` its error, ``goal [B]`` and ``seed [B]`` (int32) the
+    goal it solved toward and the seed it started from, ``steps [B]`` the rounds the group ran,
+    ``status [B]`` the OR of the winner's step statuses (0 if it ran none), ``converged [B]`` =
+    ``error <= tol``.  ``q`` carries a gradient as in :class:`Convergence`, to the winning goal's
+    row of ``goals``."""
+
+    q: torch.Tensor
+    error: torch.Tensor
+    goal: torch.Tensor
+    seed: torch.Tensor
+    steps: torch.Tensor
+    status: torch.Tensor
+    converged: torch.Tensor
+
+
 SEED_COUNTS = (1, 2, 4, 8, 16, 32)
 
 
@@ -83,6 +100,14 @@ class _SolutionOfTargets(torch.autograd.Function):
         targets, q_star, ok = ctx.saved_tensors
         grad_targets, _ = ctx.solver.converge_vjp(q_star, targets.detach(), grad_q.float().contiguous())
         return torch.where(ok[:, None], grad_targets, torch.zeros_like(grad_targets)), None, None, None
+
+
+def _solution_of_goals(goals, goal, solver, q_star, ok):
+    """``q*`` as a function of ``goals [B, G, stride]``: :class:`_SolutionOfTargets` of the
+    winning goal's row, gathered by a differentiable index, so the gradient reaches that row
+    alone."""
+    row = goals[torch.arange(goals.shape[0], device=goals.device), goal.long()]
+    return _SolutionOfTargets.apply(row, solver, q_star, ok)
 
 
 class BatchedIK:
@@ -489,6 +514,88 @@ class BatchedIK:
         if grad:
             q_out = _SolutionOfTargets.apply(targets, self, q_out, self._solved(error, status, tol))
         return MultistartConvergence(q_out, error, seed, steps, status, error <= tol)
+
+    def converge_goalset(self, q_seeds: torch.Tensor, goals: torch.Tensor, tasks: Iterable, tol: float,
+                         max_steps: int, q_out: Optional[torch.Tensor] = None, error: Optional[torch.Tensor] = None,
+                         goal: Optional[torch.Tensor] = None, seed: Optional[torch.Tensor] = None,
+                         steps: Optional[torch.Tensor] = None,
+                         status: Optional[torch.Tensor] = None) -> GoalsetConvergence:
+        """Solve each instance toward the best of several goals, from several seeds, in one launch,
+        stopping an instance as soon as one of its (goal, seed) members converges.
+
+        ``q_seeds [B, S, nq]``: as in :meth:`converge_multistart`; every goal starts from the
+        same S seeds.  ``goals [B, G, target_stride]``: G complete targets rows per instance (the
+        layout ``target_layout`` describes), so a goal may change any per-instance target;
+        shared targets stay shared.  G and S are powers of two with ``G * S`` one of 1, 2, 4, 8,
+        16, 32 (at most 8 on the tree kernel, whose ``G * S`` warp workspaces must also fit one
+        CTA's shared memory).  To use a goal count that is not a power of two, pad ``goals`` by
+        repeating one of them: a duplicate never changes the winner, since ties go to the lower
+        index.  ``tasks``, ``tol`` and ``max_steps`` as :meth:`converge`.
+
+        Member ``j = g * S + s`` starts at ``q_seeds[b, s]`` and solves toward ``goals[b, g]``.
+        The G*S members form one group of :meth:`converge_multistart`'s rule: they advance in
+        lockstep rounds, the group stops when some member has ``err <= tol``, at ``max_steps``,
+        or when every member has failed, and the winner is the member with the smallest error at
+        the stopping round (NaN counts as +inf; ties go to the lowest ``j``: the earlier goal,
+        then the earlier seed, so goals may be listed in order of preference).  The result gives
+        ``goal = j // S`` and ``seed = j % S``.
+
+        With G = 1 the result equals :meth:`converge_multistart`'s.  With S = 1, every instance
+        that :meth:`converge` from ``q_seeds[:, 0]`` solves toward some goal is solved here too,
+        in at most the smallest of those step counts.  With ``goals.requires_grad`` (and grad mode
+        on) the returned ``q`` carries the gradient with respect to the winning goal's row
+        (the other rows get zero; so do instances that did not converge), under the conditions
+        of :meth:`converge`.  Asynchronous on the current stream; no allocation inside the
+        library, so the call can be captured in a CUDA graph.  ``q_seeds`` is only read and must
+        not overlap ``q_out``."""
+        eng = self.engine
+        mask, tol = self._stop_test(tasks, tol, max_steps)
+        grad = self._grad_mode(goals, mask)
+        if (q_seeds.dim() != 3 or q_seeds.shape[2] != self.nq or q_seeds.dtype != torch.float32
+                or not q_seeds.is_contiguous()):
+            raise ValueError(f"q_seeds must be a contiguous float32 [B, S, {self.nq}] tensor")
+        B, S = int(q_seeds.shape[0]), int(q_seeds.shape[1])
+        T = self.target_stride
+        if goals is None or goals.dim() != 3 or goals.shape[0] != B or goals.shape[2] != T:
+            shape = None if goals is None else tuple(goals.shape)
+            raise ValueError(f"goals has shape {shape}, expected ({B}, G, {T})")
+        G = int(goals.shape[1])
+        if goals.dtype != torch.float32:
+            raise ValueError(f"goals must be float32, got {goals.dtype}")
+        if T > 0 and (goals.stride(2) != 1 or goals.stride(1) != T or goals.stride(0) != G * T):
+            raise ValueError("goals rows must be contiguous, target_stride floats apart")
+        if G not in SEED_COUNTS:
+            raise ValueError(f"the number of goals must be one of {SEED_COUNTS} (pad by repeating a goal), got {G}")
+        if S not in SEED_COUNTS:
+            raise ValueError(f"the number of seeds must be one of {SEED_COUNTS}, got {S}")
+        if G * S > SEED_COUNTS[-1]:
+            raise ValueError(f"goals x seeds must be at most {SEED_COUNTS[-1]}, got {G} x {S}")
+        lib = eng.lib
+        # the path-dependent limits on G S (the tree kernel's): the library validates a call with
+        # no targets without launching anything
+        if lib.pk_converge_goalset_prepared(eng.handle, self._handle, None, S, None, G, mask, tol, int(max_steps),
+                                            None, None, None, None, None, None, 0, None):
+            raise ValueError("pink_b200: " + lib.pk_last_error().decode("utf-8", "replace"))
+        if q_out is None:
+            q_out = torch.empty((B, self.nq), device=eng.device, dtype=torch.float32)
+        if error is None:
+            error = torch.empty((B,), device=eng.device, dtype=torch.float32)
+        if goal is None:
+            goal = torch.empty((B,), device=eng.device, dtype=torch.int32)
+        if seed is None:
+            seed = torch.empty((B,), device=eng.device, dtype=torch.int32)
+        if steps is None:
+            steps = torch.empty((B,), device=eng.device, dtype=torch.int32)
+        if status is None:
+            status = torch.empty((B,), device=eng.device, dtype=torch.int32)
+        with torch.cuda.device(eng.device):
+            _cabi.check(lib.pk_converge_goalset_prepared(
+                eng.handle, self._handle, _addr(q_seeds), S, _addr(goals), G, mask, tol, int(max_steps),
+                _addr(q_out), _addr(error), _addr(goal), _addr(seed), _addr(steps), _addr(status), B,
+                _stream(eng.device)))
+        if grad:
+            q_out = _solution_of_goals(goals, goal, self, q_out, self._solved(error, status, tol))
+        return GoalsetConvergence(q_out, error, goal, seed, steps, status, error <= tol)
 
     def sample_seeds(self, q: torch.Tensor, num_seeds: int, generator: Optional[torch.Generator] = None) -> torch.Tensor:
         """Seeds for :meth:`converge_multistart`: ``q [B, nq]`` -> ``[B, num_seeds, nq]``.

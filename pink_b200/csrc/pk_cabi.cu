@@ -1268,43 +1268,56 @@ extern "C" int pk_converge_prepared(const PkModel* m, const PkProblem* pr, const
   });
 }
 
-extern "C" int pk_converge_multistart_prepared(const PkModel* m, const PkProblem* pr, const float* q_seeds,
-                                               int32_t num_seeds, const float* targets, uint32_t task_mask, float tol,
-                                               int32_t max_steps, float* q_out, float* err, int32_t* seed,
-                                               int32_t* steps, int32_t* status, int64_t B, void* stream_) {
+extern "C" int pk_converge_goalset_prepared(const PkModel* m, const PkProblem* pr, const float* q_seeds,
+                                            int32_t num_seeds, const float* targets, int32_t num_goals,
+                                            uint32_t task_mask, float tol, int32_t max_steps, float* q_out, float* err,
+                                            int32_t* goal, int32_t* seed, int32_t* steps, int32_t* status, int64_t B,
+                                            void* stream_) {
   if (check_prepared(m, pr, q_seeds, targets, B, [&] {
         const std::string aerr = pk::check_converge_args(pr->P, task_mask, tol, max_steps);
         if (!aerr.empty()) return fail(aerr);
-        const std::string serr = pk::check_multistart_seeds(pr->sel, num_seeds);
+        const std::string serr = pk::check_goalset_members(pr->sel, num_goals, num_seeds);
         if (!serr.empty()) return fail(serr);
-        if (B > (int64_t)2147483647 * 32 / num_seeds) return fail("batch too large");
+        if (B > (int64_t)2147483647 * 32 / (num_goals * num_seeds)) return fail("batch too large");
         return B > 0 && !q_out ? fail("null q_out") : 0;
       }))
     return 1;
   if (B == 0) return 0;
   const pk::Selection& sel = pr->sel;
-  const int S = num_seeds;
+  const int S = num_seeds, G = num_goals;
   cudaStream_t stream = (cudaStream_t)stream_;
   if (sel.path == pk::kPathTree) {
     if (B > 2147483647) return fail("batch too large");
     const pk::MultistartTreeLayout T = pk::multistart_tree_layout(sel.plan);
-    return launch_tree(pk::ik_tree_multistart_kernel, g_tree_multistart_smem, m, B, 32 * S, T.smem_bytes(S), stream,
-                       m->dev, pr->P, T.plan, T.o_v, T.o_q, q_seeds, S, targets, task_mask, tol, (int)max_steps,
-                       q_out, err, seed, steps, status, B);
+    return launch_tree(pk::ik_tree_multistart_kernel, g_tree_multistart_smem, m, B, 32 * G * S, T.smem_bytes(G * S),
+                       stream, m->dev, pr->P, T.plan, T.o_v, T.o_q, q_seeds, S, targets, G, task_mask, tol,
+                       (int)max_steps, q_out, err, goal, seed, steps, status, B);
   }
   if (sel.path == pk::kPathChain) {
     const unsigned emask = pk::chain_task_mask(pr->P, task_mask, sel.nft);
     return pk::with_chain(sel, [&](auto nj, auto nft) {
-      constexpr int NJ = decltype(nj)::value;
-      return launch_rows(pk::ik_chain_multistart_kernel<NJ, decltype(nft)::value>, B * S, 128, stream, pr->chain<NJ>(),
-                         q_seeds, S, targets, emask, tol, (int)max_steps, q_out, err, seed, steps, status, B);
+      constexpr int NJ = decltype(nj)::value, NFT = decltype(nft)::value;
+      auto launch = [&](auto kernel) {
+        return launch_rows(kernel, B * G * S, 128, stream, pr->chain<NJ>(), q_seeds, S, targets, G, emask, tol,
+                           (int)max_steps, q_out, err, goal, seed, steps, status, B);
+      };
+      return G == 1 ? launch(pk::ik_chain_multistart_kernel<NJ, NFT, false>)
+                    : launch(pk::ik_chain_multistart_kernel<NJ, NFT, true>);
     });
   }
   return pk::with_generic(sel.generic_class, [&](auto nj, auto nv) {
-    return launch_rows(pk::ik_generic_multistart_kernel<decltype(nj)::value, decltype(nv)::value>, B * S, 64, stream,
-                       m->dev, pr->P, q_seeds, S, targets, task_mask, tol, (int)max_steps, q_out, err, seed, steps,
-                       status, B);
+    return launch_rows(pk::ik_generic_multistart_kernel<decltype(nj)::value, decltype(nv)::value>, B * G * S, 64,
+                       stream, m->dev, pr->P, q_seeds, S, targets, G, task_mask, tol, (int)max_steps, q_out, err, goal,
+                       seed, steps, status, B);
   });
+}
+
+extern "C" int pk_converge_multistart_prepared(const PkModel* m, const PkProblem* pr, const float* q_seeds,
+                                               int32_t num_seeds, const float* targets, uint32_t task_mask, float tol,
+                                               int32_t max_steps, float* q_out, float* err, int32_t* seed,
+                                               int32_t* steps, int32_t* status, int64_t B, void* stream_) {
+  return pk_converge_goalset_prepared(m, pr, q_seeds, num_seeds, targets, 1, task_mask, tol, max_steps, q_out, err,
+                                      nullptr, seed, steps, status, B, stream_);
 }
 
 extern "C" int pk_converge_vjp_prepared(const PkModel* m, const PkProblem* pr, const float* q_star,

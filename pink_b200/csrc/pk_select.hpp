@@ -103,11 +103,12 @@ inline ConvergeTreeLayout converge_tree_layout(const TreePlan& plan) {
   return T;
 }
 
-// Multi-start on joint trees (pk_converge_multistart_prepared): one target per CTA, one seed per
-// warp.  A warp's workspace is converge's, then the seed's q (4-word aligned); after the S
-// workspaces come the group's slots, two rounds of S errors and S failed flags.  The CTA's
-// dynamic shared memory is capped at kCtaSmemBytes, the opt-in limit of sm_90.
-constexpr int kTreeMaxSeeds = 8;
+// Goal-set and multi-start solves on joint trees (pk_converge_goalset_prepared): one instance per
+// CTA, one member (goal, seed) per warp.  A warp's workspace is converge's, then the member's q
+// (4-word aligned); after the workspaces of the S members (goals x seeds) come the group's
+// slots, two rounds of S errors and S failed flags.  The CTA's dynamic shared memory is capped at
+// kCtaSmemBytes, the opt-in limit of sm_90.
+constexpr int kTreeMaxSeeds = 8;  // members per CTA
 constexpr size_t kCtaSmemBytes = 227 * 1024;
 struct MultistartTreeLayout : ConvergeTreeLayout {
   int o_q;
@@ -120,17 +121,27 @@ inline MultistartTreeLayout multistart_tree_layout(const TreePlan& plan) {
   return T;
 }
 
-// Arguments of pk_converge_multistart_prepared beyond check_converge_args; "" when valid.
-inline std::string check_multistart_seeds(const Selection& sel, int S) {
-  if (!valid_num_seeds(S)) return "num_seeds must be 1, 2, 4, 8, 16 or 32";
+// Arguments of pk_converge_multistart_prepared beyond check_converge_args; "" when valid.  `what`
+// names S in the messages (the members of a goal set, check_goalset_members).
+inline std::string check_multistart_seeds(const Selection& sel, int S, const std::string& what = "num_seeds") {
+  if (!valid_num_seeds(S)) return what + " must be 1, 2, 4, 8, 16 or 32";
   if (sel.path == kPathTree) {
-    if (S > kTreeMaxSeeds) return "num_seeds must be at most 8 on the tree kernel (one warp per seed in one CTA)";
+    if (S > kTreeMaxSeeds) return what + " must be at most 8 on the tree kernel (one warp each in one CTA)";
     const size_t bytes = multistart_tree_layout(sel.plan).smem_bytes(S);
     if (bytes > kCtaSmemBytes)
-      return "num_seeds = " + std::to_string(S) + " needs " + std::to_string(bytes) +
+      return what + " = " + std::to_string(S) + " needs " + std::to_string(bytes) +
              " B of shared memory on the tree kernel, more than one CTA's " + std::to_string(kCtaSmemBytes) + " B";
   }
   return "";
+}
+
+// Arguments of pk_converge_goalset_prepared beyond check_converge_args: G goals and S seeds, each
+// a power of two, whose G S members form one multi-start group; "" when valid.
+inline std::string check_goalset_members(const Selection& sel, int G, int S) {
+  if (G == 1) return check_multistart_seeds(sel, S);
+  if (!valid_num_seeds(G)) return "num_goals must be 1, 2, 4, 8, 16 or 32";
+  if (!valid_num_seeds(S)) return "num_seeds must be 1, 2, 4, 8, 16 or 32";
+  return check_multistart_seeds(sel, G * S, "num_goals * num_seeds");
 }
 
 // Problems pk_converge_vjp_prepared differentiates: tasks, the box limits and FloatingBaseVelocityLimit
