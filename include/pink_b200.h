@@ -326,6 +326,32 @@ int pk_converge_goalset_prepared(const PkModel* model, const PkProblem* problem,
                                  float* err, int32_t* goal, int32_t* seed, int32_t* steps,
                                  int32_t* status, int64_t B, void* stream);
 
+/* Solve to separate position and orientation tolerances: pk_converge_prepared with another
+ * err(q), the largest over the tasks of task_mask of
+ *   frame, relative frame   max(|e[0:3]|, (tol / orientation_tol) |e[3:6]|),
+ *   CoM, linear (holonomic, joint coupling)   |e|,
+ *   posture                 |e|,
+ * where e is the task's unweighted, gain-free error (log6's twist for a pose) restricted to the
+ * rows whose cost is > 0: an instance stops when every weighed translation part is <= tol, every
+ * weighed rotation part (the rotation angle when all three axes are weighed) is <= orientation_tol
+ * and every other task is <= tol.  orientation_tol = +inf leaves the rotation rows out of the
+ * test.  tol must be finite and > 0, orientation_tol > 0, and every task of task_mask must keep a
+ * row to test.  The loop, the step, the outputs and the launch are those of pk_converge_prepared. */
+int pk_converge_pose_tol_prepared(const PkModel* model, const PkProblem* problem,
+                                  const float* q, const float* targets, uint32_t task_mask, float tol,
+                                  float orientation_tol, int32_t max_steps, float* q_out, float* err,
+                                  int32_t* steps, int32_t* status, int64_t B, void* stream);
+
+/* Goal-set (and, with num_goals = 1, multi-start) solve to separate position and orientation
+ * tolerances: pk_converge_goalset_prepared with the err(q) of pk_converge_pose_tol_prepared; the
+ * rounds, the winner's order and the outputs are unchanged.                                  */
+int pk_converge_goalset_pose_tol_prepared(const PkModel* model, const PkProblem* problem,
+                                          const float* q_seeds, int32_t num_seeds, const float* targets,
+                                          int32_t num_goals, uint32_t task_mask, float tol,
+                                          float orientation_tol, int32_t max_steps, float* q_out,
+                                          float* err, int32_t* goal, int32_t* seed, int32_t* steps,
+                                          int32_t* status, int64_t B, void* stream);
+
 /* Gradient of a loss with respect to the targets at solutions of pk_converge_prepared /
  * pk_converge_multistart_prepared: grad_targets[b] = (d q_star / d T)^T grad_q[b] at q_star[b]
  * (targets[B][target_stride] the rows the solutions were converged to, grad_q[B][nq] the loss

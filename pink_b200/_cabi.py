@@ -201,6 +201,11 @@ def declare(lib: C.CDLL, prefix: str = "pk_") -> None:
     lib.pk_converge_goalset_prepared.argtypes = [C.c_void_p, C.c_void_p, _FP, C.c_int32, _FP, C.c_int32, C.c_uint32,
                                                  C.c_float, C.c_int32, _FP, _FP, _FP, _FP, _FP, _FP, C.c_int64,
                                                  C.c_void_p]
+    lib.pk_converge_pose_tol_prepared.argtypes = [C.c_void_p, C.c_void_p, _FP, _FP, C.c_uint32, C.c_float, C.c_float,
+                                                  C.c_int32, _FP, _FP, _FP, _FP, C.c_int64, C.c_void_p]
+    lib.pk_converge_goalset_pose_tol_prepared.argtypes = [C.c_void_p, C.c_void_p, _FP, C.c_int32, _FP, C.c_int32,
+                                                          C.c_uint32, C.c_float, C.c_float, C.c_int32, _FP, _FP, _FP,
+                                                          _FP, _FP, _FP, C.c_int64, C.c_void_p]
     lib.pk_converge_vjp_prepared.argtypes = [C.c_void_p, C.c_void_p, _FP, _FP, _FP, _FP, _FP, C.c_int64, C.c_void_p]
     lib.pk_build_ik_batched.argtypes = [C.c_void_p, C.POINTER(PkProblemDesc), _FP, _FP, _FP, _FP, _FP, C.c_int64, C.c_void_p]
     lib.pk_constraint_rows_batched.argtypes = [C.c_void_p, C.POINTER(PkProblemDesc), _FP, _FP, _FP, _FP, _FP, _FP, _FP, _FP, C.c_int64, C.c_void_p]
@@ -238,6 +243,8 @@ EXPORTED_SYMBOLS = [
     "pk_converge_prepared",
     "pk_converge_multistart_prepared",
     "pk_converge_goalset_prepared",
+    "pk_converge_pose_tol_prepared",
+    "pk_converge_goalset_pose_tol_prepared",
     "pk_converge_vjp_prepared",
     "pk_build_ik_batched",
     "pk_constraint_rows_batched",

@@ -12,6 +12,7 @@ launch through ``pk_solve_ik_prepared``.
 from __future__ import annotations
 
 import ctypes as C
+import math
 from typing import Iterable, NamedTuple, Optional
 
 import torch
@@ -303,7 +304,8 @@ class BatchedIK:
 
     def converge(self, q: torch.Tensor, targets: Optional[torch.Tensor], tasks: Iterable, tol: float,
                  max_steps: int, q_out: Optional[torch.Tensor] = None, error: Optional[torch.Tensor] = None,
-                 steps: Optional[torch.Tensor] = None, status: Optional[torch.Tensor] = None) -> Convergence:
+                 steps: Optional[torch.Tensor] = None, status: Optional[torch.Tensor] = None,
+                 orientation_tol: Optional[float] = None) -> Convergence:
         """Solve each instance to a tolerance in one launch: the loop of the reference's
         ``examples/inverse_kinematics_ur10.py`` (``while norm(task.compute_error(c)) > thres``).
 
@@ -324,11 +326,20 @@ class BatchedIK:
         with respect to ``targets``, one :meth:`converge_vjp` launch in the backward pass, zero
         for instances that did not converge.  Every frame, relative frame and CoM task must then
         be in ``tasks`` (so that ``tol`` bounds the gradient's error), and problems with barriers,
-        constraints or ``AccelerationLimit`` are rejected (``ValueError``)."""
+        constraints or ``AccelerationLimit`` are rejected (``ValueError``).
+
+        ``orientation_tol`` selects separate position and orientation tolerances: a task's error
+        then counts only the components it weighs (cost > 0), and a frame or relative-frame task's
+        is ``max(|e[0:3]|, (tol / orientation_tol) |e[3:6]|)``, so ``error <= tol`` means every
+        weighed translation part is within ``tol`` (metres), every weighed rotation part within
+        ``orientation_tol`` (radians) and every other task within ``tol``.  ``inf`` leaves
+        orientations out of the test.  A position-only task (``orientation_cost=0``) can then
+        converge and be differentiated (DESIGN.md section 3.2h)."""
         eng = self.engine
         B = q.shape[0]
         mask, tol = self._stop_test(tasks, tol, max_steps)
-        grad = self._grad_mode(targets, mask)
+        orientation_tol = self._orientation_tol(mask, tol, orientation_tol)
+        grad = self._grad_mode(targets, mask, orientation_tol)
         if tuple(q.shape) != (B, self.nq) or q.dtype != torch.float32 or not q.is_contiguous():
             raise ValueError(f"q must be a contiguous float32 [B, {self.nq}] tensor")
         self._check_fixed_targets(targets, B)
@@ -341,9 +352,14 @@ class BatchedIK:
         if status is None:
             status = torch.empty((B,), device=eng.device, dtype=torch.int32)
         with torch.cuda.device(eng.device):
-            _cabi.check(eng.lib.pk_converge_prepared(eng.handle, self._handle, _addr(q), _addr(targets), mask, tol,
-                                                     int(max_steps), _addr(q_out), _addr(error), _addr(steps),
-                                                     _addr(status), B, _stream(eng.device)))
+            if orientation_tol is None:
+                _cabi.check(eng.lib.pk_converge_prepared(eng.handle, self._handle, _addr(q), _addr(targets), mask, tol,
+                                                         int(max_steps), _addr(q_out), _addr(error), _addr(steps),
+                                                         _addr(status), B, _stream(eng.device)))
+            else:
+                _cabi.check(eng.lib.pk_converge_pose_tol_prepared(
+                    eng.handle, self._handle, _addr(q), _addr(targets), mask, tol, orientation_tol, int(max_steps),
+                    _addr(q_out), _addr(error), _addr(steps), _addr(status), B, _stream(eng.device)))
         if grad:
             q_out = _SolutionOfTargets.apply(targets, self, q_out, self._solved(error, status, tol))
         return Convergence(q_out, error, steps, status, error <= tol)
@@ -400,11 +416,16 @@ class BatchedIK:
                                                          _stream(eng.device)))
         return grad_targets, status
 
-    def _grad_mode(self, targets: Optional[torch.Tensor], mask: int) -> bool:
+    def _grad_mode(self, targets: Optional[torch.Tensor], mask: int, orientation_tol: Optional[float] = None) -> bool:
         """Whether :meth:`converge` / :meth:`converge_multistart` attach the gradient with respect
-        to ``targets``; checks that the problem is one whose gradient error ``tol`` bounds."""
+        to ``targets``; checks that the problem is one whose gradient error ``tol`` bounds.  With
+        ``orientation_tol`` the components a task does not weigh are left untested: their zero
+        weight keeps them out of the gradient, so ``orientation_tol`` must only be finite."""
         if targets is None or not (torch.is_grad_enabled() and targets.requires_grad):
             return False
+        if orientation_tol is not None and not math.isfinite(orientation_tol):
+            raise ValueError("gradients of converge need a finite orientation_tol, so that the test bounds every "
+                             "weighed error")
         for k in range(len(self.tasks)):
             if int(self.prob.tasks[k].type) in (_cabi.PK_TASK_FRAME, _cabi.PK_TASK_RELATIVE_FRAME,
                                                 _cabi.PK_TASK_COM) and not (mask >> k) & 1:
@@ -445,6 +466,29 @@ class BatchedIK:
             raise ValueError(f"max_steps must be an integer >= 0, got {max_steps}")
         return mask, tol
 
+    def _orientation_tol(self, mask: int, tol: float, orientation_tol: Optional[float]) -> Optional[float]:
+        """``orientation_tol`` of :meth:`converge` and its siblings, validated (None: the default
+        test).  The separate-tolerance test checks only weighed components, so every task of the
+        mask must keep one."""
+        if orientation_tol is None:
+            return None
+        r = float(orientation_tol)
+        if not (tol > 0.0):
+            raise ValueError(f"tol must be finite and > 0 with orientation_tol, got {tol}")
+        if not (r > 0.0):
+            raise ValueError(f"orientation_tol must be > 0 (inf: orientations are not tested), got {orientation_tol}")
+        for k in range(len(self.tasks)):
+            if not (mask >> k) & 1:
+                continue
+            d = self.prob.tasks[k]
+            ty = int(d.type)
+            n = 1 if ty == _cabi.PK_TASK_POSTURE else 3 if ty == _cabi.PK_TASK_COM else \
+                int(d.rows) if ty == _cabi.PK_TASK_LINEAR else 6
+            pose = ty in (_cabi.PK_TASK_FRAME, _cabi.PK_TASK_RELATIVE_FRAME)
+            if not any(float(d.cost[i]) > 0.0 and (not pose or i < 3 or math.isfinite(r)) for i in range(n)):
+                raise ValueError(f"{self.tasks[k]!r} weighs no component the stopping test could check")
+        return r
+
     def _check_fixed_targets(self, targets: Optional[torch.Tensor], B: int) -> None:
         """One fixed targets row per instance (or target), ``[B, target_stride]``."""
         S = self.target_stride
@@ -462,7 +506,8 @@ class BatchedIK:
     def converge_multistart(self, q_seeds: torch.Tensor, targets: Optional[torch.Tensor], tasks: Iterable, tol: float,
                             max_steps: int, q_out: Optional[torch.Tensor] = None, error: Optional[torch.Tensor] = None,
                             seed: Optional[torch.Tensor] = None, steps: Optional[torch.Tensor] = None,
-                            status: Optional[torch.Tensor] = None) -> MultistartConvergence:
+                            status: Optional[torch.Tensor] = None,
+                            orientation_tol: Optional[float] = None) -> MultistartConvergence:
         """Solve each target to a tolerance from several seeds in one launch, stopping a target as
         soon as one of its seeds converges.
 
@@ -480,10 +525,12 @@ class BatchedIK:
         With S = 1 the result equals :meth:`converge`'s.  With seed 0 the caller's start, every
         target :meth:`converge` solves from it is solved here too, in at most as many steps.
         Asynchronous on the current stream; no allocation inside the library, so the call can
-        be captured in a CUDA graph.  ``q_seeds`` is only read and must not overlap ``q_out``."""
+        be captured in a CUDA graph.  ``q_seeds`` is only read and must not overlap ``q_out``.
+        ``orientation_tol`` as in :meth:`converge`."""
         eng = self.engine
         mask, tol = self._stop_test(tasks, tol, max_steps)
-        grad = self._grad_mode(targets, mask)
+        orientation_tol = self._orientation_tol(mask, tol, orientation_tol)
+        grad = self._grad_mode(targets, mask, orientation_tol)
         if (q_seeds.dim() != 3 or q_seeds.shape[2] != self.nq or q_seeds.dtype != torch.float32
                 or not q_seeds.is_contiguous()):
             raise ValueError(f"q_seeds must be a contiguous float32 [B, S, {self.nq}] tensor")
@@ -494,8 +541,14 @@ class BatchedIK:
         lib = eng.lib
         # the path-dependent limits on S (the tree kernel's): the library validates a call with no
         # targets without launching anything
-        if lib.pk_converge_multistart_prepared(eng.handle, self._handle, None, S, None, mask, tol, int(max_steps),
-                                               None, None, None, None, None, 0, None):
+        if orientation_tol is None:
+            bad = lib.pk_converge_multistart_prepared(eng.handle, self._handle, None, S, None, mask, tol,
+                                                      int(max_steps), None, None, None, None, None, 0, None)
+        else:
+            bad = lib.pk_converge_goalset_pose_tol_prepared(eng.handle, self._handle, None, S, None, 1, mask, tol,
+                                                            orientation_tol, int(max_steps), None, None, None, None,
+                                                            None, None, 0, None)
+        if bad:
             raise ValueError("pink_b200: " + lib.pk_last_error().decode("utf-8", "replace"))
         if q_out is None:
             q_out = torch.empty((B, self.nq), device=eng.device, dtype=torch.float32)
@@ -508,9 +561,15 @@ class BatchedIK:
         if status is None:
             status = torch.empty((B,), device=eng.device, dtype=torch.int32)
         with torch.cuda.device(eng.device):
-            _cabi.check(lib.pk_converge_multistart_prepared(
-                eng.handle, self._handle, _addr(q_seeds), S, _addr(targets), mask, tol, int(max_steps), _addr(q_out),
-                _addr(error), _addr(seed), _addr(steps), _addr(status), B, _stream(eng.device)))
+            if orientation_tol is None:
+                _cabi.check(lib.pk_converge_multistart_prepared(
+                    eng.handle, self._handle, _addr(q_seeds), S, _addr(targets), mask, tol, int(max_steps),
+                    _addr(q_out), _addr(error), _addr(seed), _addr(steps), _addr(status), B, _stream(eng.device)))
+            else:  # multi-start is the goal-set solve with one goal
+                _cabi.check(lib.pk_converge_goalset_pose_tol_prepared(
+                    eng.handle, self._handle, _addr(q_seeds), S, _addr(targets), 1, mask, tol, orientation_tol,
+                    int(max_steps), _addr(q_out), _addr(error), None, _addr(seed), _addr(steps), _addr(status), B,
+                    _stream(eng.device)))
         if grad:
             q_out = _SolutionOfTargets.apply(targets, self, q_out, self._solved(error, status, tol))
         return MultistartConvergence(q_out, error, seed, steps, status, error <= tol)
@@ -519,7 +578,8 @@ class BatchedIK:
                          max_steps: int, q_out: Optional[torch.Tensor] = None, error: Optional[torch.Tensor] = None,
                          goal: Optional[torch.Tensor] = None, seed: Optional[torch.Tensor] = None,
                          steps: Optional[torch.Tensor] = None,
-                         status: Optional[torch.Tensor] = None) -> GoalsetConvergence:
+                         status: Optional[torch.Tensor] = None,
+                         orientation_tol: Optional[float] = None) -> GoalsetConvergence:
         """Solve each instance toward the best of several goals, from several seeds, in one launch,
         stopping an instance as soon as one of its (goal, seed) members converges.
 
@@ -547,10 +607,11 @@ class BatchedIK:
         (the other rows get zero; so do instances that did not converge), under the conditions
         of :meth:`converge`.  Asynchronous on the current stream; no allocation inside the
         library, so the call can be captured in a CUDA graph.  ``q_seeds`` is only read and must
-        not overlap ``q_out``."""
+        not overlap ``q_out``.  ``orientation_tol`` as in :meth:`converge`."""
         eng = self.engine
         mask, tol = self._stop_test(tasks, tol, max_steps)
-        grad = self._grad_mode(goals, mask)
+        orientation_tol = self._orientation_tol(mask, tol, orientation_tol)
+        grad = self._grad_mode(goals, mask, orientation_tol)
         if (q_seeds.dim() != 3 or q_seeds.shape[2] != self.nq or q_seeds.dtype != torch.float32
                 or not q_seeds.is_contiguous()):
             raise ValueError(f"q_seeds must be a contiguous float32 [B, S, {self.nq}] tensor")
@@ -573,8 +634,14 @@ class BatchedIK:
         lib = eng.lib
         # the path-dependent limits on G S (the tree kernel's): the library validates a call with
         # no targets without launching anything
-        if lib.pk_converge_goalset_prepared(eng.handle, self._handle, None, S, None, G, mask, tol, int(max_steps),
-                                            None, None, None, None, None, None, 0, None):
+        if orientation_tol is None:
+            bad = lib.pk_converge_goalset_prepared(eng.handle, self._handle, None, S, None, G, mask, tol,
+                                                   int(max_steps), None, None, None, None, None, None, 0, None)
+        else:
+            bad = lib.pk_converge_goalset_pose_tol_prepared(eng.handle, self._handle, None, S, None, G, mask, tol,
+                                                            orientation_tol, int(max_steps), None, None, None, None,
+                                                            None, None, 0, None)
+        if bad:
             raise ValueError("pink_b200: " + lib.pk_last_error().decode("utf-8", "replace"))
         if q_out is None:
             q_out = torch.empty((B, self.nq), device=eng.device, dtype=torch.float32)
@@ -589,10 +656,16 @@ class BatchedIK:
         if status is None:
             status = torch.empty((B,), device=eng.device, dtype=torch.int32)
         with torch.cuda.device(eng.device):
-            _cabi.check(lib.pk_converge_goalset_prepared(
-                eng.handle, self._handle, _addr(q_seeds), S, _addr(goals), G, mask, tol, int(max_steps),
-                _addr(q_out), _addr(error), _addr(goal), _addr(seed), _addr(steps), _addr(status), B,
-                _stream(eng.device)))
+            if orientation_tol is None:
+                _cabi.check(lib.pk_converge_goalset_prepared(
+                    eng.handle, self._handle, _addr(q_seeds), S, _addr(goals), G, mask, tol, int(max_steps),
+                    _addr(q_out), _addr(error), _addr(goal), _addr(seed), _addr(steps), _addr(status), B,
+                    _stream(eng.device)))
+            else:
+                _cabi.check(lib.pk_converge_goalset_pose_tol_prepared(
+                    eng.handle, self._handle, _addr(q_seeds), S, _addr(goals), G, mask, tol, orientation_tol,
+                    int(max_steps), _addr(q_out), _addr(error), _addr(goal), _addr(seed), _addr(steps),
+                    _addr(status), B, _stream(eng.device)))
         if grad:
             q_out = _solution_of_goals(goals, goal, self, q_out, self._solved(error, status, tol))
         return GoalsetConvergence(q_out, error, goal, seed, steps, status, error <= tol)

@@ -18,6 +18,7 @@
 #include "pk_coop_kernel.cuh"
 #include "pk_generic.cuh"
 #include "pk_multistart.cuh"
+#include "pk_pose_tol.hpp"
 #include "pk_select.hpp"
 
 namespace {
@@ -634,8 +635,7 @@ __global__ void __launch_bounds__(64)
 }
 
 // Tree kernel: one instance per warp, per-instance state in the warp's slice of
-// dynamic shared memory (pk_tree.cuh).
-constexpr int kTreeWarpsPerBlock = 2;
+// dynamic shared memory (pk_tree.cuh); kTreeWarpsPerBlock in pk_select.hpp.
 // resident CTAs per SM the register allocation aims at: 10 (96 registers, 40 B of spills) ran
 // 4 % faster than 8 (128 registers) on configs 3 / 4 (scripts/r2_tree_ab.sh)
 #ifndef PK_TREE_MIN_BLOCKS
@@ -1236,11 +1236,22 @@ extern "C" int pk_rollout_trajectory_prepared(const PkModel* m, const PkProblem*
   });
 }
 
-extern "C" int pk_converge_prepared(const PkModel* m, const PkProblem* pr, const float* q, const float* targets,
-                                    uint32_t task_mask, float tol, int32_t max_steps, float* q_out, float* err,
-                                    int32_t* steps, int32_t* status, int64_t B, void* stream_) {
+namespace {
+
+// Stopping test of a converge call: the default one (pose = false), or separate position and
+// orientation tolerances (pk_converge_pose_tol_prepared), whose kernels pk_pose_tol.cu launches.
+struct StopMode {
+  bool pose = false;
+  float orientation_tol = 0.f;
+};
+
+// The launch of pk_converge_prepared and pk_converge_pose_tol_prepared.
+int launch_converge(const PkModel* m, const PkProblem* pr, const float* q, const float* targets, uint32_t task_mask,
+             float tol, int32_t max_steps, float* q_out, float* err, int32_t* steps, int32_t* status, int64_t B,
+             void* stream_, const StopMode& mode) {
   if (check_prepared(m, pr, q, targets, B, [&] {
-        const std::string aerr = pk::check_converge_args(pr->P, task_mask, tol, max_steps);
+        std::string aerr = pk::check_converge_args(pr->P, task_mask, tol, max_steps);
+        if (aerr.empty() && mode.pose) aerr = pk::check_pose_tol_args(pr->P, task_mask, tol, mode.orientation_tol);
         if (!aerr.empty()) return fail(aerr);
         return B > 0 && !q_out ? fail("null q_out") : 0;
       }))
@@ -1248,13 +1259,20 @@ extern "C" int pk_converge_prepared(const PkModel* m, const PkProblem* pr, const
   if (B == 0) return 0;
   cudaStream_t stream = (cudaStream_t)stream_;
   const pk::Selection& sel = pr->sel;
+  if (mode.pose) {
+    const pk::PoseTolLaunch a{&sel, m->dev, &pr->P, pr->chain_params, m->device, q, 1, targets, 1, task_mask, tol,
+                              mode.orientation_tol, (int)max_steps, q_out, err, nullptr, nullptr, steps, status, B,
+                              stream};
+    PK_CUDA(pk::launch_converge_pose_tol(a));
+    return launched();
+  }
   if (sel.path == pk::kPathChain) {
     // always the thread-per-instance kernel: PK_CHAIN_LANES selects only the solve entries' variant
     const unsigned emask = pk::chain_task_mask(pr->P, task_mask, sel.nft);
     return pk::with_chain(sel, [&](auto nj, auto nft) {
-      constexpr int NJ = decltype(nj)::value;
-      return launch_rows(pk::ik_chain_converge_kernel<NJ, decltype(nft)::value>, B, 128, stream, pr->chain<NJ>(), q,
-                         targets, emask, tol, (int)max_steps, q_out, err, steps, status, B);
+      constexpr int NJ = decltype(nj)::value, NFT = decltype(nft)::value;
+      return launch_rows(pk::ik_chain_converge_kernel<NJ, NFT>, B, 128, stream, pr->chain<NJ>(), q, targets, emask, tol,
+                         (int)max_steps, q_out, err, steps, status, B);
     });
   }
   if (sel.path == pk::kPathTree) {
@@ -1263,18 +1281,20 @@ extern "C" int pk_converge_prepared(const PkModel* m, const PkProblem* pr, const
                              T.plan, T.o_v, q, targets, task_mask, tol, (int)max_steps, q_out, err, steps, status, B);
   }
   return pk::with_generic(sel.generic_class, [&](auto nj, auto nv) {
-    return launch_rows(pk::ik_generic_converge_kernel<decltype(nj)::value, decltype(nv)::value>, B, 64, stream, m->dev,
-                       pr->P, q, targets, task_mask, tol, (int)max_steps, q_out, err, steps, status, B);
+    constexpr int NJ = decltype(nj)::value, NV = decltype(nv)::value;
+    return launch_rows(pk::ik_generic_converge_kernel<NJ, NV>, B, 64, stream, m->dev, pr->P, q, targets, task_mask, tol,
+                       (int)max_steps, q_out, err, steps, status, B);
   });
 }
 
-extern "C" int pk_converge_goalset_prepared(const PkModel* m, const PkProblem* pr, const float* q_seeds,
-                                            int32_t num_seeds, const float* targets, int32_t num_goals,
-                                            uint32_t task_mask, float tol, int32_t max_steps, float* q_out, float* err,
-                                            int32_t* goal, int32_t* seed, int32_t* steps, int32_t* status, int64_t B,
-                                            void* stream_) {
+// The launch of pk_converge_goalset_prepared and pk_converge_goalset_pose_tol_prepared.
+int launch_converge_goalset(const PkModel* m, const PkProblem* pr, const float* q_seeds, int32_t num_seeds,
+                     const float* targets, int32_t num_goals, uint32_t task_mask, float tol, int32_t max_steps,
+                     float* q_out, float* err, int32_t* goal, int32_t* seed, int32_t* steps, int32_t* status,
+                     int64_t B, void* stream_, const StopMode& mode) {
   if (check_prepared(m, pr, q_seeds, targets, B, [&] {
-        const std::string aerr = pk::check_converge_args(pr->P, task_mask, tol, max_steps);
+        std::string aerr = pk::check_converge_args(pr->P, task_mask, tol, max_steps);
+        if (aerr.empty() && mode.pose) aerr = pk::check_pose_tol_args(pr->P, task_mask, tol, mode.orientation_tol);
         if (!aerr.empty()) return fail(aerr);
         const std::string serr = pk::check_goalset_members(pr->sel, num_goals, num_seeds);
         if (!serr.empty()) return fail(serr);
@@ -1286,8 +1306,14 @@ extern "C" int pk_converge_goalset_prepared(const PkModel* m, const PkProblem* p
   const pk::Selection& sel = pr->sel;
   const int S = num_seeds, G = num_goals;
   cudaStream_t stream = (cudaStream_t)stream_;
+  if (sel.path == pk::kPathTree && B > 2147483647) return fail("batch too large");
+  if (mode.pose) {
+    const pk::PoseTolLaunch a{&sel, m->dev, &pr->P, pr->chain_params, m->device, q_seeds, S, targets, G, task_mask, tol,
+                              mode.orientation_tol, (int)max_steps, q_out, err, goal, seed, steps, status, B, stream};
+    PK_CUDA(pk::launch_goalset_pose_tol(a));
+    return launched();
+  }
   if (sel.path == pk::kPathTree) {
-    if (B > 2147483647) return fail("batch too large");
     const pk::MultistartTreeLayout T = pk::multistart_tree_layout(sel.plan);
     return launch_tree(pk::ik_tree_multistart_kernel, g_tree_multistart_smem, m, B, 32 * G * S, T.smem_bytes(G * S),
                        stream, m->dev, pr->P, T.plan, T.o_v, T.o_q, q_seeds, S, targets, G, task_mask, tol,
@@ -1306,10 +1332,45 @@ extern "C" int pk_converge_goalset_prepared(const PkModel* m, const PkProblem* p
     });
   }
   return pk::with_generic(sel.generic_class, [&](auto nj, auto nv) {
-    return launch_rows(pk::ik_generic_multistart_kernel<decltype(nj)::value, decltype(nv)::value>, B * G * S, 64,
-                       stream, m->dev, pr->P, q_seeds, S, targets, G, task_mask, tol, (int)max_steps, q_out, err, goal,
-                       seed, steps, status, B);
+    constexpr int NJ = decltype(nj)::value, NV = decltype(nv)::value;
+    return launch_rows(pk::ik_generic_multistart_kernel<NJ, NV>, B * G * S, 64, stream, m->dev, pr->P, q_seeds, S,
+                       targets, G, task_mask, tol, (int)max_steps, q_out, err, goal, seed, steps, status, B);
   });
+}
+
+}  // namespace
+
+extern "C" int pk_converge_prepared(const PkModel* m, const PkProblem* pr, const float* q, const float* targets,
+                                    uint32_t task_mask, float tol, int32_t max_steps, float* q_out, float* err,
+                                    int32_t* steps, int32_t* status, int64_t B, void* stream_) {
+  return launch_converge(m, pr, q, targets, task_mask, tol, max_steps, q_out, err, steps, status, B, stream_, StopMode{});
+}
+
+extern "C" int pk_converge_pose_tol_prepared(const PkModel* m, const PkProblem* pr, const float* q,
+                                             const float* targets, uint32_t task_mask, float tol,
+                                             float orientation_tol, int32_t max_steps, float* q_out, float* err,
+                                             int32_t* steps, int32_t* status, int64_t B, void* stream_) {
+  return launch_converge(m, pr, q, targets, task_mask, tol, max_steps, q_out, err, steps, status, B, stream_,
+                  StopMode{true, orientation_tol});
+}
+
+extern "C" int pk_converge_goalset_prepared(const PkModel* m, const PkProblem* pr, const float* q_seeds,
+                                            int32_t num_seeds, const float* targets, int32_t num_goals,
+                                            uint32_t task_mask, float tol, int32_t max_steps, float* q_out, float* err,
+                                            int32_t* goal, int32_t* seed, int32_t* steps, int32_t* status, int64_t B,
+                                            void* stream_) {
+  return launch_converge_goalset(m, pr, q_seeds, num_seeds, targets, num_goals, task_mask, tol, max_steps, q_out, err, goal,
+                          seed, steps, status, B, stream_, StopMode{});
+}
+
+extern "C" int pk_converge_goalset_pose_tol_prepared(const PkModel* m, const PkProblem* pr, const float* q_seeds,
+                                                     int32_t num_seeds, const float* targets, int32_t num_goals,
+                                                     uint32_t task_mask, float tol, float orientation_tol,
+                                                     int32_t max_steps, float* q_out, float* err, int32_t* goal,
+                                                     int32_t* seed, int32_t* steps, int32_t* status, int64_t B,
+                                                     void* stream_) {
+  return launch_converge_goalset(m, pr, q_seeds, num_seeds, targets, num_goals, task_mask, tol, max_steps, q_out, err, goal,
+                          seed, steps, status, B, stream_, StopMode{true, orientation_tol});
 }
 
 extern "C" int pk_converge_multistart_prepared(const PkModel* m, const PkProblem* pr, const float* q_seeds,

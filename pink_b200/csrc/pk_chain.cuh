@@ -83,9 +83,11 @@ struct ChainStep {
   // tasks of `emask` in chain slots (bit k < NFT: ft[k], bit NFT: the posture task).  An
   // instance outside its limits still runs the forward kinematics then, because its error is
   // wanted too; it returns right after the task errors.
-  template <bool ERR = false>
+  // POSE: a frame task's error is pose_err over the axes of `amask` (bit 6 k + r: row r of ft[k];
+  // chain_axis_mask) with rscale = tol / orientation_tol, the separate-tolerance test.
+  template <bool ERR = false, bool POSE = false>
   PK_HD int assemble(const ChainParams<NJ>& P, const float (&q)[NJ], const float* __restrict__ trow, bool& skip,
-                     unsigned emask = 0u, float* err = nullptr) {
+                     unsigned emask = 0u, float* err = nullptr, unsigned amask = 0u, float rscale = 0.f) {
   int status = 0;
   float emax = 0.f;
 #pragma unroll
@@ -147,7 +149,17 @@ struct ChainStep {
     Log3 L = log3(Tbt.R);
     float e[6];
     log6(Tbt, L, e);
-    if constexpr (ERR) {
+    if constexpr (ERR && POSE) {
+      if ((emask >> t) & 1u) {
+        float l2 = 0.f, a2 = 0.f;
+#pragma unroll
+        for (int k = 0; k < 3; ++k) {
+          if ((amask >> (6 * t + k)) & 1u) l2 = fmaf(e[k], e[k], l2);
+          if ((amask >> (6 * t + 3 + k)) & 1u) a2 = fmaf(e[3 + k], e[3 + k], a2);
+        }
+        emax = err_max(emax, pose_err(l2, a2, rscale));
+      }
+    } else if constexpr (ERR) {
       if ((emask >> t) & 1u) {
         float n2 = 0.f;
 #pragma unroll
@@ -319,9 +331,11 @@ PK_HD bool converge_chain_advance(const ChainParams<NJ>& P, ChainStep<NJ, NFT>& 
 // q_s when err <= tol or s == max_steps; otherwise take the step ik_step_chain takes (its status
 // ORed into status_out), stop at q_s if the freeze rule of the rollouts fires, and move to
 // q_s (+) v dt.  On return q is where the instance stopped, err its error, steps the solves.
-template <int NJ, int NFT>
+// POSE, amask, rscale: the separate-tolerance test (ChainStep::assemble).
+template <int NJ, int NFT, bool POSE = false>
 PK_HD void converge_chain(const ChainParams<NJ>& P, float (&q)[NJ], const float* __restrict__ trow, unsigned emask,
-                          float tol, int max_steps, float& err, int& steps, int& status_out, int flags = 0) {
+                          float tol, int max_steps, float& err, int& steps, int& status_out, int flags = 0,
+                          unsigned amask = 0u, float rscale = 0.f) {
   int st_all = 0;
   int s = 0;
 #pragma unroll 1
@@ -329,7 +343,7 @@ PK_HD void converge_chain(const ChainParams<NJ>& P, float (&q)[NJ], const float*
     ChainStep<NJ, NFT> C;
     bool skip;
     float e;
-    const int status = C.template assemble<true>(P, q, trow, skip, emask, &e);
+    const int status = C.template assemble<true, POSE>(P, q, trow, skip, emask, &e, amask, rscale);
     err = e;
     if (e <= tol || s == max_steps) break;
     if (!converge_chain_advance(P, C, status, skip, q, st_all, flags)) {
@@ -343,17 +357,19 @@ PK_HD void converge_chain(const ChainParams<NJ>& P, float (&q)[NJ], const float*
 
 // Instance i of ik_chain_converge_kernel: converge_chain from q row i, where it stopped into q_out
 // row i, then err, steps and status (each unless null).  q_out may alias q (the row is read before
-// it is written).
-template <int NJ, int NFT>
+// it is written).  POSE, amask, rscale: as converge_chain.
+template <int NJ, int NFT, bool POSE = false>
 PK_HD void converge_chain_instance(const ChainParams<NJ>& P, const float* q, const float* __restrict__ targets,
                                    unsigned emask, float tol, int max_steps, float* q_out, float* __restrict__ err,
-                                   int32_t* __restrict__ steps, int32_t* __restrict__ status, int64_t i) {
+                                   int32_t* __restrict__ steps, int32_t* __restrict__ status, int64_t i,
+                                   unsigned amask = 0u, float rscale = 0.f) {
   float qi[NJ];
 #pragma unroll
   for (int k = 0; k < NJ; ++k) qi[k] = q[i * NJ + k];
   float e;
   int n, st;
-  converge_chain<NJ, NFT>(P, qi, targets + i * (int64_t)P.target_stride, emask, tol, max_steps, e, n, st);
+  converge_chain<NJ, NFT, POSE>(P, qi, targets + i * (int64_t)P.target_stride, emask, tol, max_steps, e, n, st, 0,
+                                amask, rscale);
 #pragma unroll
   for (int k = 0; k < NJ; ++k) q_out[i * NJ + k] = qi[k];
   if (err) err[i] = e;

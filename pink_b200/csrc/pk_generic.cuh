@@ -448,6 +448,7 @@ struct Generic {
   // ERR (converge_generic): also the stop test `ct` on the task errors, made before the QP; a
   // step that stops there writes only *out.status (and ct).  Test: the stop rule, ct->decide(err)
   // (ConvergeTest: this instance's own; the multi-start kernel's decides for a group of seeds).
+  // Test::kPose (PoseTolTest): a non-diagonal task's error is task_pose_err with ct->rot_scale.
   template <bool ERR = false, class Test = ConvergeTest>
   PK_HD void step(const DevModel& M, const DevProblem& P, const float* q, const float* trow, const GenericOut& out,
                   Test* ct = nullptr) {
@@ -526,7 +527,12 @@ struct Generic {
       }
       float e[6];
       const int k = task_rows(M, P, Kt, q, tgt, e, Jw);
-      if constexpr (ERR) {
+      if constexpr (ERR && Test::kPose) {
+        if ((ct->mask >> t) & 1u) {
+          const bool pose = Kt.type == PK_TASK_FRAME || Kt.type == PK_TASK_RELATIVE_FRAME;
+          emax = err_max(emax, task_pose_err(pose, e, Kt.cost, k, ct->rot_scale));
+        }
+      } else if constexpr (ERR) {
         if ((ct->mask >> t) & 1u) {
           float n2 = 0.f;
           for (int r = 0; r < k; ++r) n2 = fmaf(e[r], e[r], n2);
@@ -898,11 +904,11 @@ struct Generic {
 
 // Solve to a tolerance (pk_converge_prepared), one instance on the general path; the loop of
 // converge_chain (pk_chain.cuh) with Generic::step.  q [nq]: in q_0, out where the instance
-// stopped (updated in place); v [nv]: scratch.
-template <int NJMAX, int NVMAX>
+// stopped (updated in place); v [nv]: scratch.  POSE, rot_scale: the separate-tolerance test.
+template <int NJMAX, int NVMAX, bool POSE = false>
 PK_HD void converge_generic(Generic<NJMAX, NVMAX>& G, const DevModel& M, const DevProblem& P, float* q,
                             const float* trow, float* v, unsigned mask, float tol, int max_steps, float& err,
-                            int& steps, int& status_out) {
+                            int& steps, int& status_out, float rot_scale = 0.f) {
   int32_t st = 0;
   GenericOut out{};
   out.v = v;
@@ -912,7 +918,13 @@ PK_HD void converge_generic(Generic<NJMAX, NVMAX>& G, const DevModel& M, const D
   int s = 0;
   for (;; ++s) {
     ConvergeTest ct{mask, tol, s == max_steps, 0.f, false, 0};
-    G.template step<true>(M, P, q, trow, out, &ct);
+    if constexpr (POSE) {
+      PoseTolTest<ConvergeTest> pt{ct, rot_scale};
+      G.template step<true>(M, P, q, trow, out, &pt);
+      ct = pt;
+    } else {
+      G.template step<true>(M, P, q, trow, out, &ct);
+    }
     err = ct.err;
     if (ct.stop) break;
     st_all |= st;
@@ -970,20 +982,20 @@ PK_HD void rollout_generic_instance(Generic<NJMAX, NVMAX>& G, const DevModel& M,
 
 // Instance i of ik_generic_converge_kernel: q row i into q_out row i (q_out may alias q),
 // converge_generic there in place with v in local memory, then err, steps and status (each unless
-// null).
-template <int NJMAX, int NVMAX>
+// null).  POSE, rot_scale: as converge_generic.
+template <int NJMAX, int NVMAX, bool POSE = false>
 PK_HD void converge_generic_instance(Generic<NJMAX, NVMAX>& G, const DevModel& M, const DevProblem& P, const float* q,
                                      const float* __restrict__ targets, unsigned mask, float tol, int max_steps,
                                      float* q_out, float* __restrict__ err, int32_t* __restrict__ steps,
-                                     int32_t* __restrict__ status, int64_t i) {
+                                     int32_t* __restrict__ status, int64_t i, float rot_scale = 0.f) {
   const int nq = M.nq;
   float* qrow = q_out + i * nq;
   for (int k = 0; k < nq; ++k) qrow[k] = q[i * nq + k];
   float v[NVMAX];
   float e;
   int n, st;
-  converge_generic(G, M, P, qrow, targets ? targets + i * (int64_t)P.target_stride : nullptr, v, mask, tol, max_steps,
-                   e, n, st);
+  converge_generic<NJMAX, NVMAX, POSE>(G, M, P, qrow, targets ? targets + i * (int64_t)P.target_stride : nullptr, v,
+                                       mask, tol, max_steps, e, n, st, rot_scale);
   if (err) err[i] = e;
   if (steps) steps[i] = n;
   if (status) status[i] = st;

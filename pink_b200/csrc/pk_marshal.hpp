@@ -191,6 +191,24 @@ inline std::string check_converge_args(const DevProblem& P, uint32_t mask, float
   return "";
 }
 
+// Arguments of pk_converge_pose_tol_prepared beyond check_converge_args'; "" when valid.  The
+// test only checks rows with cost > 0 (a frame task's rotation rows only for a finite
+// orientation_tol), so every task of the mask must keep one.
+inline std::string check_pose_tol_args(const DevProblem& P, uint32_t mask, float tol, float orientation_tol) {
+  if (!(tol > 0.f) || !std::isfinite(tol)) return "tol must be finite and > 0 with orientation_tol";
+  if (!(orientation_tol > 0.f)) return "orientation_tol must be > 0 (inf: orientations are not tested)";
+  for (int t = 0; t < P.ntasks; ++t) {
+    if (!((mask >> t) & 1u)) continue;
+    const DevTask& d = P.tasks[t];
+    const bool pose = d.type == PK_TASK_FRAME || d.type == PK_TASK_RELATIVE_FRAME;
+    const int k = is_diag_task(d.type) ? 1 : d.type == PK_TASK_COM ? 3 : d.type == PK_TASK_LINEAR ? d.rows : 6;
+    bool any = false;
+    for (int r = 0; r < k; ++r) any = any || (d.cost[r] > 0.f && (!pose || r < 3 || orientation_tol < INFINITY));
+    if (!any) return "task " + std::to_string(t) + " of the task mask has no weighed component left to test";
+  }
+  return "";
+}
+
 // Seeds per target of pk_converge_multistart_prepared (and goals, and goals x seeds, of
 // pk_converge_goalset_prepared): a power of two that fits one warp, so that a group is S
 // adjacent lanes.

@@ -517,7 +517,9 @@ PK_HD float err_max(float m, float n) { return (n > m || n != n) ? n : m; }
 // (the step then returns before its QP), and the step's status (the same on every lane).
 // The bodies take the test type as a template parameter: decide() is the stop rule, called
 // where the error is known (the multi-start kernels pass a test that decides for a group).
+// kPose selects the error at compile time: false here, true in PoseTolTest.
 struct ConvergeTest {
+  static constexpr bool kPose = false;
   unsigned mask;
   float tol;
   bool last;
@@ -529,6 +531,41 @@ struct ConvergeTest {
     stop = e <= tol || last;
   }
 };
+
+// A stop test (ConvergeTest or a multi-start kernel's group test) under separate position and
+// orientation tolerances (pk_converge_pose_tol_prepared): the step bodies take each task's error
+// from task_pose_err (the chain's from pose_err), with rot_scale = tol / orientation_tol.  A type
+// of its own, with the mode a compile-time constant, so that the bodies' default instantiations
+// and the test types' layouts are those of the default test.
+template <class Test>
+struct PoseTolTest : Test {
+  static constexpr bool kPose = true;
+  float rot_scale;
+};
+
+// Error of one pose task under separate position and orientation tolerances
+// (pk_converge_pose_tol_prepared): lin2 and ang2 are the squared norms of log6's translation and
+// rotation parts on the axes the task weighs, rs = tol / orientation_tol (0: orientation_tol =
+// inf, the rotation part is not tested).  err <= tol exactly when the translation part is <= tol
+// and the rotation part <= orientation_tol; a NaN stays NaN.
+PK_HD float pose_err(float lin2, float ang2, float rs) { return err_max(sqrtf(lin2), rs * sqrtf(ang2)); }
+
+// err_t of the separate-tolerance test from a task's rows e[0, k) and its costs (DevTask.cost):
+// only the rows with cost > 0 are tested; frame and relative-frame tasks split them by pose_err,
+// CoM and linear tasks take the norm of the tested rows.  The diagonal tasks (posture) are
+// tested by their whole norm, as in the default test.
+PK_HD float task_pose_err(bool pose, const float* e, const float* cost, int k, float rs) {
+  float lin2 = 0.f, ang2 = 0.f;
+  for (int r = 0; r < k; ++r) {
+    if (!(cost[r] > 0.f)) continue;
+    if (pose && r >= 3) {
+      if (rs > 0.f) ang2 = fmaf(e[r], e[r], ang2);
+    } else {
+      lin2 = fmaf(e[r], e[r], lin2);
+    }
+  }
+  return pose ? pose_err(lin2, ang2, rs) : sqrtf(lin2);
+}
 
 // Order of the seeds of a multi-start group (pk_converge_multistart_prepared): seed a (error ea)
 // comes before seed b when its error is smaller, a NaN error counting as +inf, ties going to the

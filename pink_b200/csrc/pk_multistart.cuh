@@ -16,6 +16,8 @@
 // lanes; joint trees run one instance per CTA, one member per warp.  The bodies whose stop test
 // sits in the middle of the step (Generic::step, TreeStep::run) take a test type whose decide()
 // makes the group's decision there.
+//
+// Their siblings under separate position and orientation tolerances are in pk_pose_tol.cu.
 #pragma once
 
 #include "pk_chain.cuh"
@@ -48,6 +50,7 @@ __device__ __forceinline__ int group_winner(unsigned lanes, int S, float e, int 
 // Group stop test over the lanes of a group (Generic::step).  A failed member still calls the
 // step (its lanes take part in the votes) and keeps the error it had where it failed.
 struct LaneGroupTest {
+  static constexpr bool kPose = false;
   unsigned mask;
   float tol;
   bool last;
@@ -70,6 +73,7 @@ struct LaneGroupTest {
 // reached by all of them; the slots alternate between two rounds, so a warp that runs ahead
 // cannot overwrite slots another warp has yet to read.
 struct CtaGroupTest {
+  static constexpr bool kPose = false;
   unsigned mask;
   float tol;
   bool last;
@@ -200,6 +204,7 @@ __global__ void __launch_bounds__(64)
   if (status) status[b] = st_all;
 }
 
+#ifndef PK_NO_TREE_MULTISTART_KERNEL  // pk_pose_tol.cu: a translation unit of other kernels
 // Joint trees: instance b = blockIdx.x, member j = warp, blockDim = 32 G S.  Warp j's workspace
 // (MultistartTreeLayout) holds the plan's words, the step's v at o_v and the member's q at o_q;
 // the group's slots follow the G S workspaces.  All warps run the same rounds (CtaGroupTest), and
@@ -260,5 +265,6 @@ __global__ void __launch_bounds__(32 * kTreeMaxSeeds)
     if (status) status[b] = st_all;
   }
 }
+#endif
 
 }  // namespace pk

@@ -91,6 +91,26 @@ inline unsigned chain_task_mask(const DevProblem& P, unsigned mask, int nft) {
   return out;
 }
 
+// The axes the separate-tolerance test (pk_converge_pose_tol_prepared) checks on the chain
+// kernels, per frame slot: bit 6 f + r when frame task f is in `mask` and weighs row r (cost > 0),
+// the rotation rows only for a finite orientation_tol.  Computed once per launch, so that the
+// step tests no cost.
+inline unsigned chain_axis_mask(const DevProblem& P, unsigned mask, float orientation_tol) {
+  unsigned out = 0u;
+  int f = 0;
+  for (int t = 0; t < P.ntasks; ++t) {
+    if (P.tasks[t].type != PK_TASK_FRAME) continue;
+    if ((mask >> t) & 1u)
+      for (int r = 0; r < 6; ++r)
+        if (P.tasks[t].cost[r] > 0.f && (r < 3 || orientation_tol < INFINITY)) out |= 1u << (6 * f + r);
+    ++f;
+  }
+  return out;
+}
+
+// Warps (instances) per CTA of the one-instance-per-warp tree kernels.
+constexpr int kTreeWarpsPerBlock = 2;
+
 // Solve to a tolerance on joint trees (pk_converge_prepared): a warp's workspace is the plan's
 // words, then the step's v (4-word aligned).
 struct ConvergeTreeLayout {

@@ -631,7 +631,8 @@ struct TreeStep {
   // before the rows of A; a step that stops there, or whose instance is outside its limits with
   // safety_break, returns with v = 0.  ct->status is the step's status on every lane.  Test: the
   // stop rule, ct->decide(err), called by the whole warp (ConvergeTest: this instance's own; the
-  // multi-start kernel's decides for the CTA's group of seeds, with a barrier).
+  // multi-start kernel's decides for the CTA's group of seeds, with a barrier).  Test::kPose
+  // (PoseTolTest): a non-diagonal task's error is task_pose_err with ct->rot_scale.
   template <bool ERR = false, class Test = ConvergeTest>
   static PK_HD void run(const DevModel& M, const DevProblem& P, const TreePlan& L, const float* __restrict__ qg,
                         const float* __restrict__ tg, float* W, float* __restrict__ vg, int32_t* status_out,
@@ -813,8 +814,14 @@ struct TreeStep {
         } else {
           const float* F = W + L.o_tf + kTreeTaskWords * t;
           const int k = (Kt.type == PK_TASK_COM) ? 3 : (Kt.type == PK_TASK_LINEAR ? Kt.rows : 6);
-          #pragma unroll 1
-          for (int r = 0; r < k; ++r) n2 = fmaf(F[30 + r], F[30 + r], n2);
+          if constexpr (Test::kPose) {
+            const bool pose = Kt.type == PK_TASK_FRAME || Kt.type == PK_TASK_RELATIVE_FRAME;
+            emax = err_max(emax, task_pose_err(pose, F + 30, Kt.cost, k, ct->rot_scale));
+            continue;
+          } else {
+            #pragma unroll 1
+            for (int r = 0; r < k; ++r) n2 = fmaf(F[30 + r], F[30 + r], n2);
+          }
         }
         emax = err_max(emax, sqrtf(n2));
       }
@@ -1174,16 +1181,23 @@ struct TreeStep {
   // Solve to a tolerance (pk_converge_prepared), one instance per warp; the loop of
   // converge_chain (pk_chain.cuh) with run<true>.  qg [nq]: in q_0, out where the instance stopped
   // (updated in place by lane 0); vg [nv]: scratch.  err, steps and status are the same on every
-  // lane, so the warp leaves the loop together.
+  // lane, so the warp leaves the loop together.  POSE, rot_scale: the separate-tolerance test.
+  template <bool POSE = false>
   static PK_HD void converge(const DevModel& M, const DevProblem& P, const TreePlan& L, float* qg, const float* tg,
                              float* W, float* vg, unsigned mask, float tol, int max_steps, float& err, int& steps,
-                             int& status_out) {
+                             int& status_out, float rot_scale = 0.f) {
     int st_all = 0;
     int s = 0;
     #pragma unroll 1
     for (;; ++s) {
       ConvergeTest ct{mask, tol, s == max_steps, 0.f, false, 0};
-      run<true>(M, P, L, qg, tg, W, vg, nullptr, &ct);
+      if constexpr (POSE) {
+        PoseTolTest<ConvergeTest> pt{ct, rot_scale};
+        run<true>(M, P, L, qg, tg, W, vg, nullptr, &pt);
+        ct = pt;
+      } else {
+        run<true>(M, P, L, qg, tg, W, vg, nullptr, &ct);
+      }
       PK_WSYNC();
       err = ct.err;
       if (ct.stop) break;
@@ -1255,18 +1269,20 @@ struct TreeStep {
 
   // ik_tree_converge_kernel: q row i into q_out row i (q_out may alias q), converge there in place
   // with the step's v at word o_v of W (converge_tree_layout), then err, steps and status (each
-  // unless null).
+  // unless null).  POSE, rot_scale: as converge.
+  template <bool POSE = false>
   static PK_HD void converge_instance(const DevModel& M, const DevProblem& P, const TreePlan& L, int o_v,
                                       const float* q, const float* __restrict__ targets, unsigned mask, float tol,
                                       int max_steps, float* q_out, float* W, float* __restrict__ err,
-                                      int32_t* __restrict__ steps, int32_t* __restrict__ status, int64_t i) {
+                                      int32_t* __restrict__ steps, int32_t* __restrict__ status, int64_t i,
+                                      float rot_scale = 0.f) {
     float* qrow = q_out + i * L.nq;
     PK_LANES(l) for (int k = l; k < L.nq; k += 32) qrow[k] = q[i * L.nq + k];
     PK_WSYNC();
     float e;
     int n, st;
-    converge(M, P, L, qrow, targets ? targets + i * (int64_t)L.stride : nullptr, W, W + o_v, mask, tol, max_steps, e,
-             n, st);
+    converge<POSE>(M, P, L, qrow, targets ? targets + i * (int64_t)L.stride : nullptr, W, W + o_v, mask, tol,
+                   max_steps, e, n, st, rot_scale);
     PK_LANES(l) {
       if (l == 0) {
         if (err) err[i] = e;

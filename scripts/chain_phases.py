@@ -6,7 +6,7 @@ the per-phase instruction counts that need no GPU.
     python scripts/chain_phases.py --sass [--lib SO]                      # SASS per phase
     python scripts/chain_phases.py --paths [--batch B]                    # host build: path shares per warp
 
-GPU mode compiles an instrumented copy of the library (__graft_entry__.NVCC_FLAGS plus
+GPU mode compiles an instrumented copy of the library (__graft_entry__.compile_library with
 -DPK_CHAIN_PHASE_CLOCKS) into a temporary directory, or takes the one given with --lib, and
 loads it in place of pink_b200/libpink_b200.so.  It runs the bench.py workload (UR5, same seed,
 B = 65536, 32 rotating input sets, PDL as the library launches it) as one CUDA graph of K
@@ -41,7 +41,7 @@ import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-from __graft_entry__ import NVCC_FLAGS  # noqa: E402
+from __graft_entry__ import compile_library  # noqa: E402
 
 CSRC = os.path.join(ROOT, "pink_b200", "csrc")
 PHASES = ["entry", "loaded", "assemble", "corner", "closed_form", "rounds", "wait", "store"]
@@ -57,8 +57,7 @@ class Record(C.Structure):  # pk::ChainPhaseRecord
 
 def build_instrumented(out_dir):
     so = os.path.join(out_dir, "libpink_b200.so")
-    subprocess.check_call(["nvcc", *NVCC_FLAGS, "-DPK_CHAIN_PHASE_CLOCKS", "-o", so, os.path.join(CSRC, "pk_cabi.cu")],
-                          cwd=ROOT)
+    compile_library(ROOT, so, ["-DPK_CHAIN_PHASE_CLOCKS"])
     return so
 
 

@@ -2,8 +2,8 @@
 
     python scripts/compare_sass.py [BASE_REV] [--out DIR]
 
-Builds pink_b200/csrc/pk_cabi.cu of git revision BASE_REV (default HEAD) and of the working
-tree with __graft_entry__.NVCC_FLAGS plus -Xptxas -v, in parallel, then compares for every
+Builds the CUDA library of git revision BASE_REV (default HEAD) and of the working tree with
+__graft_entry__.compile_library plus -Xptxas -v, in parallel, then compares for every
 kernel:
   - the cuobjdump -sass listing, with the /*addr*/ comments stripped and whitespace collapsed;
   - ptxas' registers / barriers / shared and constant memory line and its stack frame / spill
@@ -22,20 +22,39 @@ import re
 import subprocess
 import sys
 import tempfile
+import threading
 from collections import defaultdict
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-from __graft_entry__ import NVCC_FLAGS  # noqa: E402
+from __graft_entry__ import compile_library  # noqa: E402
 
 ADDR = re.compile(r"/\*[0-9a-f]{4,}\*/")
+
+
+class _Build:
+    """compile_library of one source tree on a thread; wait() -> 0 on success."""
+
+    def __init__(self, src_root, so, log):
+        self.error = None
+        self.thread = threading.Thread(target=self._run, args=(src_root, so, log))
+        self.thread.start()
+
+    def _run(self, src_root, so, log):
+        try:
+            compile_library(src_root, so, ["-Xptxas", "-v"], log)
+        except Exception as exc:  # reported by wait()
+            self.error = exc
+
+    def wait(self):
+        self.thread.join()
+        return 1 if self.error else 0
 
 
 def start_build(src_root, out_dir):
     so = os.path.join(out_dir, "libpink_b200.so")
     log = open(os.path.join(out_dir, "ptxas.txt"), "w")
-    cmd = ["nvcc", *NVCC_FLAGS, "-Xptxas", "-v", "-o", so, os.path.join(src_root, "pink_b200", "csrc", "pk_cabi.cu")]
-    return so, subprocess.Popen(cmd, cwd=src_root, stdout=log, stderr=subprocess.STDOUT)
+    return so, _Build(src_root, so, log)
 
 
 def sass_by_kernel(so):
@@ -46,9 +65,14 @@ def sass_by_kernel(so):
         if m:
             name = m.group(1)
             kernels[name] = []
+        elif line.lstrip().startswith("Fatbin"):  # the next translation unit's image
+            name = None
         elif name is not None:
             # whitespace collapsed: cuobjdump pads its columns to the widest line of the whole listing
             kernels[name].append(" ".join(ADDR.sub("", line).split()))
+    for lines in kernels.values():  # the blank lines before a following image
+        while lines and not lines[-1]:
+            lines.pop()
     return kernels
 
 
