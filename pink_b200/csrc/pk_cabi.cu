@@ -443,8 +443,8 @@ __device__ __forceinline__ void chain_l2_prefetch(const float* base, int64_t n, 
 // it, so it cannot cover K rows or per-step stores: trajectory calls with a step stride or
 // records always launch <NJ, NFT, false>.  Every step's row is read through load_se3_vec4,
 // which checks each address, so a step stride that is not a multiple of 4 floats takes the
-// scalar loads.
-template <int NJ, int NFT, bool PDL>
+// scalar loads.  ARM: the problem has the arm shape (ChainParams::arm, ChainStep::assemble).
+template <int NJ, int NFT, bool PDL, bool ARM = false>
 __global__ void __launch_bounds__(128, 4)
     ik_chain_kernel(const __grid_constant__ ChainParams<NJ> P, const float* __restrict__ q,
                     const float* __restrict__ targets, float* __restrict__ v, int32_t* __restrict__ status,
@@ -477,7 +477,7 @@ __global__ void __launch_bounds__(128, 4)
   const float* const grow = targets + i * (int64_t)P.target_stride;
   int st_all;
   if constexpr (!PDL) {
-    st_all = rollout_chain<NJ, NFT, true>(P, qi, grow, vi, n_steps, q_out != nullptr, flags, T, B, i);
+    st_all = rollout_chain<NJ, NFT, true, ARM>(P, qi, grow, vi, n_steps, q_out != nullptr, flags, T, B, i);
   } else {
     using L = ChainPdlSlot<NJ, NFT>;
     const int n = P.target_stride;  // <= chain_row_words(NJ, NFT)
@@ -492,8 +492,8 @@ __global__ void __launch_bounds__(128, 4)
     PK_PHASE(kPhaseLoaded);
 #pragma unroll 1
     for (int pass = 0;; ++pass) {
-      st_all = rollout_chain<NJ, NFT, false>(P, qi, L::row() + (pass ? L::kReread : 0), vi, n_steps, q_out != nullptr,
-                                             flags, T, B, i);
+      st_all = rollout_chain<NJ, NFT, false, ARM>(P, qi, L::row() + (pass ? L::kReread : 0), vi, n_steps,
+                                                  q_out != nullptr, flags, T, B, i);
       if (pass > 0) break;
       pdl_wait();
       // the inputs as the predecessors left them; one recompute at most (nothing writes
@@ -808,10 +808,10 @@ void chain_residency(ChainResidency& r, Kernel kernel, int block, int64_t* ctas,
   }
 }
 
-template <int NJ, int NFT>
-int launch_chain(const pk::ChainParams<NJ>& C, bool pdl_row_fits, const float* q, const float* targets, float* v,
-                 int32_t* status, int64_t B, cudaStream_t stream, int n_steps, float* q_out, const pk::PeerOut& peers,
-                 const pk::Trajectory& traj) {
+template <int NJ, int NFT, bool ARM>
+int launch_chain_shape(const pk::ChainParams<NJ>& C, bool pdl_row_fits, const float* q, const float* targets, float* v,
+                       int32_t* status, int64_t B, cudaStream_t stream, int n_steps, float* q_out,
+                       const pk::PeerOut& peers, const pk::Trajectory& traj) {
   // A/B and probe switches (timing experiments; see scripts/ab.sh)
   static const int flags = (env_int("PK_CLOSED_FORM", 1) ? 0 : 1) | (env_int("PK_PROBE_SKIP_ROUNDS", 0) ? 2 : 0) |
                            (env_int("PK_CHAIN_FORCE_RECOMPUTE", 0) ? pk::kChainForceRecompute : 0);
@@ -836,19 +836,35 @@ int launch_chain(const pk::ChainParams<NJ>& C, bool pdl_row_fits, const float* q
     int l2_ctas = 0;
     if (l2_prefetch) {
       int64_t resident, l2;
-      chain_residency(residency, pk::ik_chain_kernel<NJ, NFT, true>, block, &resident, &l2);
+      chain_residency(residency, pk::ik_chain_kernel<NJ, NFT, true, ARM>, block, &resident, &l2);
       l2_ctas = pk::chain_l2_prefetch_ctas(grid, resident, B * 4 * (NJ + (int64_t)C.target_stride), l2);
     }
-    if (cudaLaunchKernelEx(&cfg, pk::ik_chain_kernel<NJ, NFT, true>, C, q, targets, v, status, B, flags, n_steps, q_out,
-                           peers, traj, l2_ctas) == cudaSuccess)
+    if (cudaLaunchKernelEx(&cfg, pk::ik_chain_kernel<NJ, NFT, true, ARM>, C, q, targets, v, status, B, flags, n_steps,
+                           q_out, peers, traj, l2_ctas) == cudaSuccess)
       return launched();
     // a driver or capture mode that rejects the attribute: plain launches from now on
     cudaGetLastError();
     g_chain_pdl_rejected.store(true, std::memory_order_relaxed);
   }
-  pk::ik_chain_kernel<NJ, NFT, false><<<(unsigned)grid, block, 0, stream>>>(C, q, targets, v, status, B, flags, n_steps,
-                                                                          q_out, peers, traj, 0);
+  pk::ik_chain_kernel<NJ, NFT, false, ARM><<<(unsigned)grid, block, 0, stream>>>(C, q, targets, v, status, B, flags,
+                                                                               n_steps, q_out, peers, traj, 0);
   return launched();
+}
+
+// the arm-shape instantiation when the problem has that shape (only with frame tasks: NFT > 0)
+template <int NJ, int NFT>
+int launch_chain(const pk::ChainParams<NJ>& C, bool pdl_row_fits, const float* q, const float* targets, float* v,
+                 int32_t* status, int64_t B, cudaStream_t stream, int n_steps, float* q_out, const pk::PeerOut& peers,
+                 const pk::Trajectory& traj) {
+  // test switch: the general instantiation for every problem (read once)
+  static const bool force_general = env_int("PK_CHAIN_FORCE_GENERAL", 0) != 0;
+  if constexpr (NFT > 0) {
+    if (C.arm && !force_general)
+      return launch_chain_shape<NJ, NFT, true>(C, pdl_row_fits, q, targets, v, status, B, stream, n_steps, q_out, peers,
+                                               traj);
+  }
+  return launch_chain_shape<NJ, NFT, false>(C, pdl_row_fits, q, targets, v, status, B, stream, n_steps, q_out, peers,
+                                            traj);
 }
 
 // size_class: pk::generic_size_class of the model

@@ -60,6 +60,9 @@ struct ChainParams {
   // AccelerationLimit (pink/limits/acceleration_limit.py:119-200): a box as well
   int acc_enabled, acc_prev_off;  // dq_prev per instance at acc_prev_off of the targets row (< 0: zeros)
   float acc_max[NJ], acc_qlo[NJ], acc_qhi[NJ];
+  // the arm shape (make_chain_params): at least one frame task, every joint revolute, every frame
+  // task on the last joint, no AccelerationLimit; ik_chain_kernel then runs ChainStep::assemble<.., ARM>
+  int arm;
 };
 
 // NFT = number of FrameTasks (compile time, so that the stacked Jacobian has a
@@ -79,13 +82,15 @@ struct ChainStep {
 
   // Returns status bits; `skip` is set when the instance must not be solved
   // (outside limits with safety_break).
+  // ARM: the problem has the arm shape (ChainParams::arm), so the joint types, the bodies of the
+  // frame tasks and acc_enabled are known at compile time; the results are bitwise those of ARM = false.
   // ERR (converge_chain): also store in *err the largest unweighted, gain-free |e_t|_2 of the
   // tasks of `emask` in chain slots (bit k < NFT: ft[k], bit NFT: the posture task).  An
   // instance outside its limits still runs the forward kinematics then, because its error is
   // wanted too; it returns right after the task errors.
   // POSE: a frame task's error is pose_err over the axes of `amask` (bit 6 k + r: row r of ft[k];
   // chain_axis_mask) with rscale = tol / orientation_tol, the separate-tolerance test.
-  template <bool ERR = false, bool POSE = false>
+  template <bool ERR = false, bool POSE = false, bool ARM = false>
   PK_HD int assemble(const ChainParams<NJ>& P, const float (&q)[NJ], const float* __restrict__ trow, bool& skip,
                      unsigned emask = 0u, float* err = nullptr, unsigned amask = 0u, float rscale = 0.f) {
   int status = 0;
@@ -108,7 +113,7 @@ struct ChainStep {
     const ChainJoint& Jn = P.joint[j];
     const SE3f X = load_se3(Jn.X);
     T = (j == 0) ? X : compose(T, X);  // T~_{-1} = I
-    if (Jn.type == PK_JOINT_REVOLUTE) {
+    if (ARM || Jn.type == PK_JOINT_REVOLUTE) {
       float s, c;
       sincos_f(q[j], &s, &c);
 #pragma unroll
@@ -125,7 +130,7 @@ struct ChainStep {
     // remember the placement of the joint that carries each task frame (selects only;
     // the frame offset is composed once, after the sweep)
 #pragma unroll
-    for (int t = 0; t < NFT; ++t) {
+    for (int t = 0; t < (ARM ? 0 : NFT); ++t) {
       const bool here = P.ft[t].body == j;
 #pragma unroll
       for (int k = 0; k < 9; ++k) Tb[t].R.m[k] = here ? T.R.m[k] : Tb[t].R.m[k];
@@ -135,7 +140,7 @@ struct ChainStep {
     }
   }
 #pragma unroll
-  for (int t = 0; t < NFT; ++t) Tf[t] = compose(Tb[t], load_se3(P.ft[t].X));
+  for (int t = 0; t < NFT; ++t) Tf[t] = compose(ARM ? T : Tb[t], load_se3(P.ft[t].X));
 
   // ---- objective in square-root form: rows of A / b are W J and W alpha e ----------
   float diag = P.damping;  // damping + sum of Levenberg-Marquardt terms
@@ -203,7 +208,7 @@ struct ChainStep {
 #pragma unroll
     for (int j = 0; j < NJ; ++j) {
       V3 tl, ta;
-      if (P.joint[j].type == PK_JOINT_REVOLUTE) {
+      if (ARM || P.joint[j].type == PK_JOINT_REVOLUTE) {
         const V3 lin = cross(wj[j], Tf[t].p - pj[j]);
         tl = mul(Pl, lin) + mul(Ql, wj[j]);
         ta = mul(Pa, wj[j]);
@@ -211,7 +216,8 @@ struct ChainStep {
         tl = mul(Pl, wj[j]);
         ta = v3(0.f, 0.f, 0.f);
       }
-      const float on = (j <= Kt.body) ? 1.f : 0.f;  // joints past the frame do not move it
+      // joints past the frame do not move it; ARM: a constant 1, whose products fold away
+      const float on = (ARM || j <= Kt.body) ? 1.f : 0.f;
       A[6 * t + 0][j] = on * tl.x;
       A[6 * t + 1][j] = on * tl.y;
       A[6 * t + 2][j] = on * tl.z;
@@ -257,7 +263,7 @@ struct ChainStep {
     hi[j] = fminf(P.cfg_gain * (P.cfg_hi[j] - q[j]), vb);
     lo[j] = fmaxf(P.cfg_gain * (P.cfg_lo[j] - q[j]), -vb);
   }
-  if (P.acc_enabled) {
+  if (!ARM && P.acc_enabled) {
     const float dt2 = P.dt * P.dt;
 #pragma unroll
     for (int j = 0; j < NJ; ++j) {
@@ -278,12 +284,12 @@ struct ChainStep {
   }
 };
 
-template <int NJ, int NFT>
+template <int NJ, int NFT, bool ARM = false>
 PK_HD void ik_step_chain(const ChainParams<NJ>& P, const float (&q)[NJ], const float* __restrict__ trow,
                          float (&v)[NJ], int& status_out, int flags = 0) {
   ChainStep<NJ, NFT> C;
   bool skip;
-  int status = C.assemble(P, q, trow, skip);
+  int status = C.template assemble<false, false, ARM>(P, q, trow, skip);
   PK_PHASE(kPhaseAssembled);
   float x[NJ];
 #pragma unroll
@@ -399,7 +405,7 @@ PK_HD void chain_record(const Trajectory& T, int s, int64_t B, int64_t i, const 
 // ran; v is the last step's.  RECORD: the targets row advances by T.target_step after every step,
 // and the records of T are stored (a frozen instance fills its remaining steps with q unchanged
 // and v = 0).
-template <int NJ, int NFT, bool RECORD>
+template <int NJ, int NFT, bool RECORD, bool ARM = false>
 PK_HD int rollout_chain(const ChainParams<NJ>& P, float (&qi)[NJ], const float* trow, float (&vi)[NJ], int n_steps,
                         bool integrate, int flags, const Trajectory& T, int64_t B, int64_t i) {
   int st_all = 0;
@@ -415,7 +421,7 @@ PK_HD int rollout_chain(const ChainParams<NJ>& P, float (&qi)[NJ], const float* 
       break;
     }
     int st;
-    ik_step_chain<NJ, NFT>(P, qi, trow, vi, st, flags);
+    ik_step_chain<NJ, NFT, ARM>(P, qi, trow, vi, st, flags);
     st_all |= st & 0xff;
     if (n_steps > 1 || integrate) {
 #pragma unroll

@@ -656,6 +656,11 @@ void make_chain_params(const HostModel& m, const DevProblem& P, ChainParams<NJ>*
     if (!C.ft[t].tgt_shared && (C.ft[t].tgt_off % 4) != 0) C.target_vec4 = 0;
   C.safety_break = P.safety_break;
   memcpy(C.shared, P.shared, sizeof(C.shared));
+  C.arm = C.n_frame_tasks > 0 && !C.acc_enabled;
+  for (int j = 0; j < NJ; ++j)
+    if (C.joint[j].type != PK_JOINT_REVOLUTE) C.arm = 0;
+  for (int t = 0; t < C.n_frame_tasks; ++t)
+    if (C.ft[t].body != NJ - 1) C.arm = 0;
 }
 
 // Parameter block of the sub-warp chain kernel (pk_coop.cuh): joint frames re-oriented so

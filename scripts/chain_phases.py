@@ -21,7 +21,7 @@ the CTAs that entered well before their launch's median CTA (--early-ns): how ma
 their blockIdx.x, their lead, how long they wait, and the load phase of those CTAs against the
 rest of the launch.
 
---sass attributes every SASS instruction of ik_chain_kernel<6, 1, true> to a phase by the
+--sass attributes every SASS instruction of ik_chain_kernel<6, 1, true, true> to a phase by the
 outermost source line of its inlining chain (nvdisasm -gi on a -lineinfo build).  --paths runs
 the host build of the kernel bodies with the PK_COUNT_ITERS hooks over the same workload and
 counts, per warp of 32 consecutive instances, which QP stages at least one lane takes.
@@ -46,7 +46,7 @@ from __graft_entry__ import compile_library  # noqa: E402
 CSRC = os.path.join(ROOT, "pink_b200", "csrc")
 PHASES = ["entry", "loaded", "assemble", "corner", "closed_form", "rounds", "wait", "store"]
 FLAGS = {"release1": 1, "release2": 2, "rounds": 4}
-KERNEL = "ik_chain_kernel<6, 1, true>"
+KERNEL = "ik_chain_kernel<6, 1, true, true>"
 MAX_WARPS = 65536  # pk::kChainPhaseMaxWarps
 
 
@@ -273,10 +273,10 @@ def sass_phases(args):
     sym = None
     for cb in cubins:
         names = subprocess.run(["cuobjdump", "-symbols", cb], capture_output=True, text=True).stdout
-        for m in re.finditer(r"(_ZN2pk\d+ik_chain_kernelILi6ELi1ELb1EE\S*)", names):
+        for m in re.finditer(r"(_ZN2pk\d+ik_chain_kernelILi6ELi1ELb1ELb1EE\S*)", names):
             sym, cubin = m.group(1), cb
     if sym is None:
-        raise RuntimeError("ik_chain_kernel<6, 1, true> not found")
+        raise RuntimeError("ik_chain_kernel<6, 1, true, true> not found")
     full = subprocess.run(["nvdisasm", "-gi", cubin], capture_output=True, text=True, check=True).stdout
     start = full.index(f".section\t.text.{sym},")
     end = full.find(".section\t", start + 1)
