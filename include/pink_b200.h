@@ -460,6 +460,22 @@ int pk_forward_kinematics_batched(const PkModel* model, const float* q,
                                   float* oMf, float* com, int64_t B,
                                   void* stream);
 
+/* Forward kinematics of selected frames, differentiable (DESIGN.md section 3.2i).
+ * frames: HOST array of num_frames frame indices (0 <= f < nframes, repeats allowed), copied into
+ * the launch; oMf[B][num_frames][12] (row-major [R | p]); com[B][3] or NULL.  0 <= num_frames <=
+ * PK_MAX_FRAMES.  Bitwise the matching rows of pk_forward_kinematics_batched.  A CoM request on a
+ * model of total mass 0 is rejected.  No allocation: the call can be captured in a CUDA graph.  */
+int pk_frame_placements_batched(const PkModel* model, const int32_t* frames, int32_t num_frames,
+                                const float* q, float* oMf, float* com, int64_t B, void* stream);
+
+/* grad_q[B][nq] = (d (oMf, com) / d q)^T (grad_oMf, grad_com), fully written; grad_oMf
+ * [B][num_frames][12] or NULL, grad_com [B][3] or NULL (NULL: that term is zero).  On a
+ * free-flyer root the quaternion's gradient is that of the normalised map (no radial part).
+ * Frames as pk_frame_placements_batched; one launch, no allocation.                           */
+int pk_frame_placements_vjp_batched(const PkModel* model, const int32_t* frames, int32_t num_frames,
+                                    const float* q, const float* grad_oMf, const float* grad_com,
+                                    float* grad_q, int64_t B, void* stream);
+
 /* Configuration.get_frame_jacobian (pink/configuration.py:203-236), LOCAL:
  * J[B][6][nv].                                                             */
 int pk_frame_jacobian_batched(const PkModel* model, int32_t frame,

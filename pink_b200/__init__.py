@@ -7,7 +7,7 @@ runs in hand-written CUDA kernels behind the C-ABI of ``include/pink_b200.h``;
 there is no CPU fallback.
 """
 
-from . import barriers, limits, tasks
+from . import barriers, kinematics, limits, tasks
 from .batched import BatchedIK
 from .collision import SphereCollisionModel
 from .configuration import Configuration
@@ -42,6 +42,7 @@ __all__ = [
     "SphereCollisionModel",
     "Task",
     "build_ik",
+    "kinematics",
     "custom_configuration_vector",
     "load_urdf",
     "solve_ik",

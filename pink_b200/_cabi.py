@@ -211,6 +211,9 @@ def declare(lib: C.CDLL, prefix: str = "pk_") -> None:
     lib.pk_constraint_rows_batched.argtypes = [C.c_void_p, C.POINTER(PkProblemDesc), _FP, _FP, _FP, _FP, _FP, _FP, _FP, _FP, C.c_int64, C.c_void_p]
     lib.pk_task_terms_batched.argtypes = [C.c_void_p, C.POINTER(PkProblemDesc), C.c_int32, _FP, _FP, _FP, _FP, C.c_int64, C.c_void_p]
     lib.pk_forward_kinematics_batched.argtypes = [C.c_void_p, _FP, _FP, _FP, C.c_int64, C.c_void_p]
+    lib.pk_frame_placements_batched.argtypes = [C.c_void_p, _FP, C.c_int32, _FP, _FP, _FP, C.c_int64, C.c_void_p]
+    lib.pk_frame_placements_vjp_batched.argtypes = [C.c_void_p, _FP, C.c_int32, _FP, _FP, _FP, _FP, C.c_int64,
+                                                    C.c_void_p]
     lib.pk_frame_jacobian_batched.argtypes = [C.c_void_p, C.c_int32, _FP, _FP, C.c_int64, C.c_void_p]
     lib.pk_integrate_batched.argtypes = [C.c_void_p, _FP, _FP, C.c_float, _FP, C.c_int64, C.c_void_p]
     lib.pk_peer_alloc.argtypes = [C.c_int, C.c_int64, C.POINTER(C.c_void_p), C.c_char_p]
@@ -250,6 +253,8 @@ EXPORTED_SYMBOLS = [
     "pk_constraint_rows_batched",
     "pk_task_terms_batched",
     "pk_forward_kinematics_batched",
+    "pk_frame_placements_batched",
+    "pk_frame_placements_vjp_batched",
     "pk_frame_jacobian_batched",
     "pk_integrate_batched",
     "pk_peer_alloc",

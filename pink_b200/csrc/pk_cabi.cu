@@ -17,6 +17,7 @@
 #include "pk_chain.cuh"
 #include "pk_coop_kernel.cuh"
 #include "pk_generic.cuh"
+#include "pk_kinematics.hpp"
 #include "pk_multistart.cuh"
 #include "pk_pose_tol.hpp"
 #include "pk_select.hpp"
@@ -1658,6 +1659,32 @@ extern "C" int pk_forward_kinematics_batched(const PkModel* m, const float* q, f
   A.com = com;
   A.task_index = -1;
   return launch_generic(m, pk::generic_size_class(m->hm), pk::kinematics_problem(), A, B, (cudaStream_t)stream);
+}
+
+extern "C" int pk_frame_placements_batched(const PkModel* m, const int32_t* frames, int32_t num_frames, const float* q,
+                                           float* oMf, float* com, int64_t B, void* stream) {
+  if (check_common(m, q, B)) return 1;
+  pk::FrameList L;
+  const std::string e = pk::make_frame_list(m->hm, frames, num_frames, com != nullptr, &L);
+  if (!e.empty()) return fail(e);
+  if (B > 0 && num_frames > 0 && !oMf) return fail("null oMf");
+  if (B == 0 || (num_frames == 0 && !com)) return 0;
+  PK_CUDA(pk::launch_frame_placements(pk::generic_size_class(m->hm), m->dev, L, q, oMf, com, B, (cudaStream_t)stream));
+  return launched();
+}
+
+extern "C" int pk_frame_placements_vjp_batched(const PkModel* m, const int32_t* frames, int32_t num_frames,
+                                               const float* q, const float* grad_oMf, const float* grad_com,
+                                               float* grad_q, int64_t B, void* stream) {
+  if (check_common(m, q, B)) return 1;
+  pk::FrameList L;
+  const std::string e = pk::make_frame_list(m->hm, frames, num_frames, grad_com != nullptr, &L);
+  if (!e.empty()) return fail(e);
+  if (B > 0 && !grad_q) return fail("null grad_q");
+  if (B == 0) return 0;
+  PK_CUDA(pk::launch_frame_placements_vjp(pk::generic_size_class(m->hm), m->dev, L, q, grad_oMf, grad_com, grad_q, B,
+                                          (cudaStream_t)stream));
+  return launched();
 }
 
 extern "C" int pk_frame_jacobian_batched(const PkModel* m, int32_t frame, const float* q, float* J, int64_t B,
